@@ -1,4 +1,4 @@
-// bundle_adjuster_b200.cc -- the B200 drop-in for src/theia/sfm/bundle_adjustment/bundle_adjuster.cc and
+// bundle_adjuster_b200.cc -- the H100 drop-in for src/theia/sfm/bundle_adjustment/bundle_adjuster.cc and
 // bundle_adjustment.cc.  Problem construction follows the reference step by step (file:line cited at each step);
 // where the reference calls into ceres::Problem to declare blocks constant / sub-parameterised, this adapter
 // records the same decision in the flattened tba_problem, and ceres::Solve (bundle_adjuster.cc:205) becomes

@@ -1,5 +1,5 @@
 // theia_compat/theia/sfm/scene.h -- Eigen-free stand-in for exactly the part of Theia's scene model that
-// bundle_adjuster.cc / bundle_adjustment.cc consume (SURVEY.md section 8b), so that the B200 adapter can be compiled
+// bundle_adjuster.cc / bundle_adjustment.cc consume (SURVEY.md section 8b), so that the adapter can be compiled
 // and tested in an image without Eigen / Ceres / glog.  Same class and method names, same storage semantics
 // (parameters are optimised IN PLACE through raw double*):
 //   Reconstruction  src/theia/sfm/reconstruction.h:66-181 (ViewIds, TrackIds, MutableView, MutableTrack,

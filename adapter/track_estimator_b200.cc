@@ -1,4 +1,4 @@
-// track_estimator_b200.cc -- TrackEstimator (src/theia/sfm/estimate_track.cc) on the B200 engine: the set of tracks to
+// track_estimator_b200.cc -- TrackEstimator (src/theia/sfm/estimate_track.cc) on the H100 engine: the set of tracks to
 // estimate is flattened once (observations in estimated views only, GetObservationsFromTrackViews :59-85), uploaded, and
 // every track runs the reference's pipeline on the device in one call.  No CPU fallback.
 #include "track_estimator_b200.h"

@@ -109,9 +109,9 @@ def run_microbench(device):
             "fp64_red_rows_gops": ex[0] if ex else None, "fp64_smem_atomic_gops": ex[1] if ex else None,
             "fp64_red_window_gops": ex[2] if ex else None,
             # gather strategies for the 48-byte camera rows, G rows/s like gather48_grows (the shipped 3 x LDG.128 lane-per-row):
-            # chunk-major loads transposed through shared memory, 64-byte padded rows with one 256-bit + one 128-bit load,
+            # chunk-major loads transposed through shared memory, 64-byte padded rows (one 128-byte line per row),
             # element-major 64-bit loads
-            "gather48_coop_grows": ex[3] if ex else None, "gather64_ld256_grows": ex[4] if ex else None,
+            "gather48_coop_grows": ex[3] if ex else None, "gather64_grows": ex[4] if ex else None,
             "gather48_elem_grows": ex[5] if ex else None,
             "how": "tba_microbench: 8 DFMA chains/thread; RED.ADD.F64 and 3xLDG.128 gathers over a 60k-double vector, "
                    "32 distinct rows per warp; best of 5 after warm-up"}
@@ -122,7 +122,7 @@ def load_peaks():
     if os.path.exists(path):
         with open(path) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
 
 
 def physical_cores():
@@ -355,7 +355,7 @@ def matcher_main(args):
     config = {"workload": "c5_matcher: %d-image sample of config 5 (10k images x 5k SIFT-128): all %d image pairs, %d x %d descriptors per pair, "
                           "ratio 0.8, symmetric, min 30 matches" % (n_img, n_img * (n_img - 1) // 2, n_desc, n_desc),
               "parallelism": "image pairs sharded round-robin over %d GPU(s), descriptors replicated, no collective" % world,
-              "l2_policy": "every step re-uploads the descriptors and streams %d candidate tiles per query block; the distance matrices are never stored; ratio test / symmetric filter on the device, only the kept matches are copied back" % ((n_desc + 127) // 128)}
+              "l2_policy": "every step re-uploads the descriptors and streams %d candidate tiles per query block; the distance matrices are never stored; ratio test / symmetric filter on the device, only the kept matches are copied back" % ((n_desc + 63) // 64)}
     sets = matcher_scene(n_img, n_desc)
     if args.impl == "reference":
         if rank != 0:
@@ -421,15 +421,17 @@ def matcher_main(args):
     if world > 1:
         dist.barrier()
     wall = allred(time.perf_counter() - t0, dist.ReduceOp.MAX if world > 1 else None)
+    if args.dump_outputs and rank == 0:
+        dump_matches(args.dump_outputs, out, moff, okb[:len(pr)])
     clocks = sampler.stop(tw0, time.time())
     dev_s = allred(1e-3 * (gemm_ms + exact_ms), dist.ReduceOp.MAX if world > 1 else None)
     gemm_s = allred(1e-3 * gemm_ms, dist.ReduceOp.MAX if world > 1 else None)
     pairs_total = len(all_pairs) * K
     n_matches = allred(float(n_matches), dist.ReduceOp.SUM if world > 1 else None)
     flops = 2.0 * n_desc * n_desc * MATCHER_DIM * 2 * len(all_pairs) * K  # both directions of every pair
-    peak = 1414.5
+    peak = 989.0
     pk = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    peak_src = "fallback"
+    peak_src = "H100 SXM data sheet (dense BF16)"
     if os.path.exists(pk):
         with open(pk) as f:
             peak = float(json.load(f)["bf16_tflops_sustained"]); peak_src = "measured (MEASURED_PEAKS.json bf16_tflops_sustained)"
@@ -446,7 +448,7 @@ def matcher_main(args):
                         "d2h_bytes_per_step": float(n_matches * 12 + len(all_pairs) * 5), "seconds": wall},
                 # per call: k_row_norms once; per chunk of <= 4M queries: k_expand_segments, k_nn_candidates, k_exact_top2, k_pair_decide, k_gather_matches
                 "gpu_launches": int(K * (1 + 5 * max(1, (len(mine) * 2 * n_desc + (4 << 20) - 1) // (4 << 20)))) * world,
-                "roofline": {"kernel": "k_nn_candidates (TF32 tcgen05.mma distance GEMM + fused top-8 epilogue from TMEM)", "bound": "tensor", "achieved": achieved,
+                "roofline": {"kernel": "k_nn_candidates (TF32 wgmma distance GEMM + fused candidate epilogue on the accumulator registers)", "bound": "tensor", "achieved": achieved,
                              "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak, "traffic": None, "peak_source": peak_src,
                              "note": "algorithmic flops 2*n1*n2*128 per direction on the TF32 path (nominal dense TF32 = half the bf16 rate the peak is quoted for); per GPU",
                              "gemm_seconds": gemm_s, "exact_seconds": allred(1e-3 * exact_ms, dist.ReduceOp.MAX if world > 1 else None)},
@@ -469,6 +471,9 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-experiments", action="store_true", help="skip the diagnostic pass over the compiled-in experiment switches")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed as DIR/<name>.npy; at N > 1 rank 0 writes "
+                         "its own part (BA: its shard of the points, matcher: its share of the image pairs)")
     ap.add_argument("--experiments-child", action="store_true", help=argparse.SUPPRESS)
     ap.add_argument("--device", type=int, default=0, help=argparse.SUPPRESS)
     args = ap.parse_args()
@@ -489,7 +494,7 @@ def main():
               "parallelism": ("points+observations sharded over %d GPU(s), cameras replicated; per PCG iteration the matvec kernel itself exchanges the partial sums over NVLink peer memory "
                                "(TBA_P2P=0: NCCL all-reduce), three NCCL all-reduces per LM iteration" % world) if world > 1 else "one GPU",
               "l2_policy": ("inputs larger than L2: the stored linearisation streamed by every kernel is %.2f GB at N=1 "
-                            "(L2 = 0.126 GB), no flush needed" if cfg["n_pt"] * cfg["obs_per_pt"] * 160 > 2 * 126e6 * world else
+                            "(L2 = 0.05 GB), no flush needed" if cfg["n_pt"] * cfg["obs_per_pt"] * 160 > 2 * 50e6 * world else
                             "WARNING: the stored linearisation (%.2f GB at N=1) is not larger than L2 per GPU at this N: "
                             "kernel times are L2-assisted") % (cfg["n_pt"] * cfg["obs_per_pt"] * 160 / 1e9)}
 
@@ -568,6 +573,7 @@ def main():
     # ---- timed: exactly K LM iterations on device-resident inputs.  Tolerances are zero, so a solve only stops early when it
     # reaches the fp64 floor of this scene (cost change exactly 0 after ~16 iterations); the remaining iterations then come
     # from further solves restarted at the initial estimate (each pays its own initial evaluation inside the timed region).
+    # A solve that makes no iteration at all ends the loop (reported in `note`).
     eng.upload(shard, engine.default_options(**solver_kwargs(K)))  # same packing, K iterations
     eng.reset_parameters(init)
     eng.set_profiling(os.environ.get("TBA_BENCH_NOPROF") is None)  # (TBA_BENCH_NOPROF=1: experiment -- what do the stage events cost? no roofline then)
@@ -575,7 +581,8 @@ def main():
     tw0 = time.time()
     t0 = time.perf_counter()
     iters, dev_s, launches_local, pcg_total, solves, s = 0, 0.0, 0.0, 0, 0, None
-    while iters < K and solves < 8:
+    step_costs = []  # cost after each timed LM iteration, over all solves of the timed region
+    while iters < K:
         if solves > 0:
             eng.reset_parameters(init)
         eng.set_max_iterations(K - iters)
@@ -585,6 +592,7 @@ def main():
         if s is None:
             s = si
         iters += got
+        step_costs.extend(si.costs[1:got + 1])
         dev_s += sum(it["iteration_time_in_seconds"] for it in si.iterations)
         launches_local += float(si.num_kernel_launches)
         pcg_total += int(si.num_linear_solver_iterations)
@@ -593,6 +601,8 @@ def main():
     barrier()
     wall = time.perf_counter() - t0
     clocks = sampler.stop(tw0, time.time())
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, eng, shard, step_costs)
     prof = eng.profile()
     stages = eng.profile_stages()
     eng.set_profiling(False)
@@ -610,15 +620,10 @@ def main():
     alg_bytes = prof["observations"] * (8 + 8 * nj) + prof["points"] * (80 + 8) + full_cam_bytes(shard)
     mv_ms = prof["matvec_ms"] / max(prof["matvec_launches"], 1)
     achieved = alg_bytes / (mv_ms * 1e-3) / 1e9 if mv_ms > 0 else 0.0
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(tpath) and args.workload == "c3_10kcam" and world == 1:  # the ncu capture is of this exact launch shape
-        with open(tpath) as f:
-            traffic = json.load(f).get("k_schur_matvec_dram_bytes_per_launch")
     lin_ms = prof["linearize_ms"] / max(prof["linearize_launches"], 1)
     lin_bytes = prof["observations"] * (8 + 16 + 8 * nj + 16) + prof["points"] * (32 + 112) + shard.n_cam * (48 + 160 + 96)
     roofline = {"kernel": "k_schur_stream<IMASK,0> (implicit Schur-complement matvec, persistent streaming kernel, one launch per PCG iteration)", "bound": "hbm",
-                "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
+                "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": None,
                 "peak_source": peak_src, "algorithmic_bytes_per_launch": alg_bytes, "avg_launch_ms": mv_ms,
                 "launches_timed": prof["matvec_launches"], "share_of_step": prof["matvec_ms"] * 1e-3 / dev_s if dev_s > 0 else None,
                 # the matvec issues 6 fp64 REDs and 1 48-byte gather per observation: floors from the measured rates
@@ -672,6 +677,43 @@ def main():
     if world > 1:
         dist.destroy_process_group()
     return 0
+
+
+DUMP_MAX_POINTS = 1_000_000  # 32 MB of homogeneous float64 points: with the cameras the dump stays well under 64 MB
+
+
+def dump_outputs(out_dir, eng, problem, step_costs):
+    """What a caller of the timed path receives after its last LM iteration: the refined cameras, intrinsics and points
+    (downloaded from the device) and the cost after each of the K timed LM iterations (one value per step, whether the
+    steps ran in one solve or in several restarted ones, so the shape is the same in every run).  Scenes with more than DUMP_MAX_POINTS points
+    keep a fixed, seeded sample of the point rows (the same rows in every run: the scene is seeded too).  At N > 1 `problem` is
+    rank 0's shard: the cameras and intrinsics are the replicated (complete) ones, the points are those of that shard."""
+    res = problem.copy()
+    eng.download(res)
+    pt = res.pt
+    if len(pt) > DUMP_MAX_POINTS:
+        pt = pt[np.sort(np.random.default_rng(0).choice(len(pt), DUMP_MAX_POINTS, replace=False))]
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in (("cameras_extrinsics", res.ext), ("intrinsics", res.intr), ("points", pt), ("costs", step_costs)):
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(a, dtype=np.float64))
+
+
+DUMP_MAX_MATCHES = 4_000_000  # 48 MB of float32 (feature1, feature2, distance) rows
+
+
+def dump_matches(out_dir, out, moff, pair_ok):
+    """What tbm_match_all returned in the last timed call: per pair the offset of its matches (match_offsets, float64) and
+    whether it passed (pair_ok, float32), and the matches themselves as float32 rows (feature1_ind, feature2_ind, distance).
+    More than DUMP_MAX_MATCHES matches keep a fixed, seeded sample of the rows."""
+    n = int(moff[-1])
+    rec = np.frombuffer(out, dtype=np.dtype([("i", "<i4"), ("j", "<i4"), ("d", "<f4")]), count=n)
+    m = np.stack([rec["i"].astype(np.float32), rec["j"].astype(np.float32), rec["d"]], axis=1) if n else np.zeros((0, 3), np.float32)
+    if n > DUMP_MAX_MATCHES:
+        m = m[np.sort(np.random.default_rng(0).choice(n, DUMP_MAX_MATCHES, replace=False))]
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "match_offsets.npy"), np.asarray(moff, dtype=np.float64))
+    np.save(os.path.join(out_dir, "pair_ok.npy"), np.asarray(pair_ok, dtype=np.float32))
+    np.save(os.path.join(out_dir, "matches.npy"), np.ascontiguousarray(m, dtype=np.float32))
 
 
 def full_cam_bytes(p):

@@ -1,5 +1,5 @@
 /*
- * theia_ba_b200.h -- C-ABI of the B200-native bundle-adjustment engine.
+ * theia_ba_b200.h -- C-ABI of the H100-native bundle-adjustment engine.
  *
  * This is the single drop-in boundary behind TheiaSfM's
  *   BundleAdjustReconstruction / BundleAdjustPartialReconstruction

@@ -17,7 +17,7 @@ def pytest_addoption(parser):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (select with -m gpu on a machine with an H100)")
     if config.getoption("--mock-engine"):
         import mock_engine_py
         mock_engine_py.install()

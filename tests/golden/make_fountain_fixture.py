@@ -1,9 +1,9 @@
-"""Generates tests/golden/fountain11_ir.npz from the reference's own fixtures
-  /root/reference/data/sfm/fountain11.bin      (a reconstruction saved by Theia after ITS OWN bundle adjustment)
-  /root/reference/data/sfm/gt_fountain11.bin   (ground-truth cameras of Strecha fountain-P11)
+"""Generates tests/golden/fountain11_ir.npz from the reference's own fixtures in a TheiaSfM checkout
+  <theia>/data/sfm/fountain11.bin      (a reconstruction saved by Theia after ITS OWN bundle adjustment)
+  <theia>/data/sfm/gt_fountain11.bin   (ground-truth cameras of Strecha fountain-P11)
 used by incremental_reconstruction_estimator_test.cc:52-160.  The reference cannot run here (C++ needing Ceres), but its
 saved OUTPUT travels: the flattened IR of that reconstruction pins our cost function against a state the reference's
-BA produced (tests/test_fountain_fixture.py).    Run:  python tests/golden/make_fountain_fixture.py
+BA produced (tests/test_fountain_fixture.py).    Run:  python tests/golden/make_fountain_fixture.py <theia checkout>
 """
 import os
 import sys
@@ -14,10 +14,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
 import theia_cereal  # noqa: E402
 
-DATA = "/root/reference/data/sfm"
-
-
 def main():
+    DATA = os.path.join(sys.argv[1], "data", "sfm")
     rec = theia_cereal.reconstruction(open(os.path.join(DATA, "fountain11.bin"), "rb").read())
     gt = theia_cereal.reconstruction(open(os.path.join(DATA, "gt_fountain11.bin"), "rb").read())
     assert rec["consumed"] == rec["total"] and gt["consumed"] == gt["total"]

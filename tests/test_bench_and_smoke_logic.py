@@ -72,11 +72,12 @@ bench.experiments_child("c1_50cam", 2, 0)
         assert set(d["stage_ms_per_step"]) >= {"matvec", "linearize", "precond_ext", "precond_intr", "rhs", "backsub", "candidate_cost"}
 
 
-def test_bench_experiments_parent_survives_a_failing_child():
-    """Without a GPU the real child cannot create an engine: every variant reports its error (or the child dies), the parent
-    returns a dictionary either way and never raises."""
+def test_bench_experiments_parent_survives_a_failing_child(monkeypatch):
+    """A child that sees no GPU (hidden from it, so that this holds on GPU machines too) cannot create an engine: every variant
+    reports its error (or the child dies), the parent returns a dictionary either way and never raises."""
     sys.path.insert(0, ROOT)
     import bench
+    monkeypatch.setenv("CUDA_VISIBLE_DEVICES", "")
     res = bench.run_experiments("c1_50cam", 1, 0, timeout=240)
     assert isinstance(res, dict) and res
     assert all(("error" in v or v.get("rc") != 0) for k, v in res.items() if k != "note") or "note" in res
@@ -114,6 +115,46 @@ bench.experiments_child("c1_50cam", 1, 0)
     for d in child:
         assert "error" not in d and d["rc"] == 0, d
     assert all(d["max_rel_cost_diff_vs_default"] <= 1e-9 for d in child[:-1] if not d["variant"].startswith("ablate"))
+
+
+def test_bench_dump_outputs_of_both_workload_kinds(tmp_path):
+    """--dump-outputs through the real ctypes bindings and the SIMT-emulation builds: the BA workload writes one cost per timed LM
+    iteration (exactly --steps of them) and the refined parameters, the matcher workload the match lists of its last call."""
+    emu = os.path.join(ROOT, "tests", "emu")
+    subprocess.check_call(["make", "-C", emu], stdout=subprocess.DEVNULL)
+    code = """
+import sys, os
+sys.path.insert(0, %r)
+import torch
+torch.cuda.set_device = lambda d: None
+torch.cuda.synchronize = lambda *a, **k: None
+from theiasfm_b200 import engine, matcher
+engine.LIB_PATH = os.path.join(%r, "libtheia_ba_b200_emu.so"); engine._LIB = None
+matcher.LIB_PATH = os.path.join(%r, "libtheia_matcher_b200_emu.so"); matcher._LIB = None
+os.environ["TBA_BENCH_MATCHER_IMAGES"] = "3"
+os.environ["TBA_BENCH_MATCHER_N"] = "40"
+import bench
+bench.run_microbench = lambda d: None
+sys.argv = ["bench.py", "--workload", "c1_50cam", "--steps", "3", "--warmup", "0", "--no-cpu-baseline", "--no-e2e", "--no-experiments",
+            "--dump-outputs", %r]
+bench.main()
+sys.argv = ["bench.py", "--workload", "c5_matcher", "--steps", "1", "--warmup", "0", "--no-cpu-baseline", "--dump-outputs", %r]
+bench.main()
+""" % (ROOT, emu, emu, str(tmp_path / "ba"), str(tmp_path / "matcher"))
+    out = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=900, cwd=ROOT)
+    assert out.returncode == 0, out.stderr[-2000:]
+    import numpy as np
+    sys.path.insert(0, ROOT)
+    from theiasfm_b200 import synthetic
+    p = synthetic.make_config("c1_50cam")
+    ba = {n: np.load(str(tmp_path / "ba" / (n + ".npy"))) for n in ("cameras_extrinsics", "intrinsics", "points", "costs")}
+    assert ba["costs"].shape == (3,) and ba["cameras_extrinsics"].shape == p.ext.shape and ba["points"].shape == p.pt.shape
+    assert ba["intrinsics"].shape == p.intr.shape and all(a.dtype == np.float64 for a in ba.values())
+    assert np.all(np.isfinite(ba["costs"])) and ba["costs"][-1] < ba["costs"][0]
+    mt = {n: np.load(str(tmp_path / "matcher" / (n + ".npy"))) for n in ("match_offsets", "pair_ok", "matches")}
+    assert mt["match_offsets"].shape == (4,) and mt["pair_ok"].shape == (3,)
+    assert mt["matches"].shape == (int(mt["match_offsets"][-1]), 3) and len(mt["matches"]) > 0
+    assert np.all(mt["matches"][:, :2] >= 0) and np.all(mt["matches"][:, :2] < 40)
 
 
 def test_smoke_against_the_emulated_engine():

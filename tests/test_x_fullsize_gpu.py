@@ -78,6 +78,6 @@ def test_full_size_trajectory_matches_oracle(oracle, workload, n_obs, iters):
     rel = np.abs(sg.costs - so.costs) / so.costs
     # accepted steps: 1e-9.  A REJECTED step's cost is the cost of an overshooting candidate far outside the region where the
     # quadratic model holds: the rounding-level difference of the two inexact PCG solutions is amplified there (2.3e-8 measured on
-    # the B200 for iteration 3 of config 2, between neighbours that agree to 7e-13 and 7e-10) -- 1e-6 for those
+    # the GPU for iteration 3 of config 2, between neighbours that agree to 7e-13 and 7e-10) -- 1e-6 for those
     assert np.all(rel[ok] <= 1e-9) and np.all(rel <= 1e-6), (sg.costs, so.costs)
     assert rel_err(pg.ext, po.ext) < 1e-6 and rel_err(pg.pt, po.pt) < 1e-6 and rel_err(pg.intr, po.intr) < 1e-6

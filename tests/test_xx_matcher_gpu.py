@@ -52,7 +52,7 @@ def test_random_descriptors_match_oracle_exactly():
 
 
 def test_tensor_core_path_equals_the_exact_kernel_at_sift_size(monkeypatch):
-    """dim 128 goes through the tcgen05 / TMA candidate pass + exact re-evaluation (tbm_matcher_tc.cuh); TBM_PATH=exact forces the
+    """dim 128 goes through the wgmma / TMA candidate pass + exact re-evaluation (tbm_matcher_tc.cuh); TBM_PATH=exact forces the
     round-1 CUDA-core kernel (bit-exact float order), the checker here: the match lists -- indices AND distances -- must be identical
     at SIFT-like sizes (non-negative unit descriptors, thousands per image, sizes that are not multiples of the 128-row tiles), with
     and without the ratio test, including an image matched against itself (zero distances, exact ties)."""

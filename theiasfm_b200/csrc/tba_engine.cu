@@ -1,4 +1,4 @@
-// tba_engine.cu -- host side of the B200 bundle-adjustment engine + the C-ABI of
+// tba_engine.cu -- host side of the H100 bundle-adjustment engine + the C-ABI of
 // include/theia_ba_b200.h.  Replaces ceres::Solve at
 // src/theia/sfm/bundle_adjustment/bundle_adjuster.cc:205: a Levenberg-Marquardt
 // trust-region loop (Ceres 1.14 TrustRegionMinimizer control flow, DESIGN.md section 3)
@@ -163,7 +163,7 @@ struct tba_context {
   DevBuf<double*> p2p_inbox_ptrs;
   DevBuf<unsigned long long*> p2p_flag_ptrs;
   unsigned long long p2p_seq = 0;
-  int n_sm = 148;
+  int n_sm = 132;
   int64_t real_matvecs = 0;  // matvec launches that did work (not early-exited after PCG convergence)
   double x_cost = 0, fixed_cost = 0;
   // host mirrors
@@ -957,8 +957,7 @@ int tba_create(int device, int rank, int world_size, const void* nccl_unique_id,
   c->pcg_fused = false;  // the emulator runs the CTAs of a launch one after the other: no grid barrier (the three phases are the same device functions)
 #endif
   { const char* e = getenv("TBA_P2P"); c->p2p_enabled = !(e != nullptr && e[0] == '0'); }
-  // round 2: the transposed RED emission and the 3-CTA/SM linearise are the defaults (driver-measured 28.1 vs 31.9 ms per
-  // LM iteration at 20 M observations, costs equal to 2e-8); TBA_TRED=0 / TBA_LIN_OCC=2 select the round-1 kernels
+  // the transposed RED emission and the 3-CTA/SM linearise are the defaults; TBA_TRED=0 / TBA_LIN_OCC=2 select the round-1 kernels
   { const char* e = getenv("TBA_LIN_OCC"); c->exp_lin_occ = !(e != nullptr && e[0] == '2'); }
   { const char* e = getenv("TBA_TRED"); c->exp_tred = !(e != nullptr && e[0] == '0'); }
   if (cudaSetDevice(device) != cudaSuccess || cudaDeviceGetAttribute(&c->n_sm, cudaDevAttrMultiProcessorCount, device) != cudaSuccess || cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking) != cudaSuccess ||
@@ -1539,7 +1538,7 @@ int tba_get_profile(tba_context* c, double* out) {
     for (auto& sp : c->ev_spans[w]) { float ms = 0; cudaEventElapsedTime(&ms, c->ev_pool[sp.first], c->ev_pool[sp.second]); tot += ms; }
     out[2 * w] = tot; out[2 * w + 1] = (double)c->ev_spans[w].size();
   }
-  out[1] = (double)c->real_matvecs;  // early-exited launches (after convergence inside a batch) cost ~2 us and do no work
+  out[1] = (double)c->real_matvecs;  // early-exited launches (after convergence inside a batch) cost one launch and do no work
   out[4] = (double)c->n_slots; out[5] = (double)c->n_obs; out[6] = (double)c->n_pt; out[7] = (double)c->NJ;
   return TBA_OK;
 }

@@ -1,4 +1,4 @@
-// tba_kernels.cuh -- sm_100a kernels of the bundle-adjustment engine.
+// tba_kernels.cuh -- sm_90a kernels of the bundle-adjustment engine.
 //
 // Replaces the arithmetic that ceres::Solve (called at
 // src/theia/sfm/bundle_adjustment/bundle_adjuster.cc:205) performs for Theia's
@@ -106,7 +106,7 @@ __device__ __forceinline__ double seg_reduce_to(double v, int run_last, int lane
 
 // fp64 reduction into GLOBAL memory without a return value.  Written as the PTX `red` itself: left to the compiler, atomicAdd
 // becomes ATOMG (with its round trip back to the SM) as soon as the kernel also contains a __threadfence -- the multi-GPU
-// epilogue of k_schur_stream made every matvec 13 % slower that way (round 2, GPU call 4: RED wavefronts 0, ATOMG instead).
+// epilogue of k_schur_stream made every matvec slower that way (SASS: no RED left, ATOMG instead).
 __device__ __forceinline__ void red_add(double* p, double v) {
 #ifdef TBA_EMULATE
   atomicAdd(p, v);
@@ -117,7 +117,7 @@ __device__ __forceinline__ void red_add(double* p, double v) {
 
 // Experiment TBA_TRED=1 ("transposed" RED emission).  A lane-per-observation RED of an N-double camera row touches 32
 // different 32-byte sectors per instruction (32 cameras), i.e. N x 32 sector operations at the L2 atomic units, which
-// is what bounds these kernels (profiles/: k_precond_ext 88 % lts throughput at one sector operation per RED).  Here
+// is what bounds these kernels (one L2 sector operation per lane and RED).  Here
 // the warp first stages its 32 rows in shared memory ([32][N] doubles, lane-major) and then emits them element-major:
 // instruction k covers elements 32k..32k+31 of the staged [32*N] array, so consecutive lanes add to consecutive doubles
 // of the same row and one RED instruction covers about 32*8/32 = 8..11 sectors instead of 32 -- the same N RED
@@ -1277,7 +1277,7 @@ k_schur_stream(DevProblem P, const double* __restrict__ xs, double* __restrict__
 //   * the SCHUR_JACOBI intrinsics blocks  Si[g] += sum_o J_i^T J_i - sum_(p,g) W^T M_p W,  W = sum_{o in p and g} J_p^T J_i
 //     (k_precond_intr; the per-(point, group) sums W by ballot-driven segmented shuffle reduction instead of shared-memory
 //     atomics; with one shared group every lane keeps its share of Si in registers until the end of its range).
-// Three sweeps over the 3.2 GB linearisation (5.7 ms at 20 M observations in round 1) become one.
+// Three sweeps over the 3.2 GB linearisation (at 20 M observations) become one.
 // Long tiles keep the three tile kernels (engine: stage_prepare).
 template <uint32_t IMASK>
 struct PrepCfg {

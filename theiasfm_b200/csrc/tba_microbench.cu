@@ -41,7 +41,7 @@ __global__ void k_gather(const double* __restrict__ x, unsigned n_rows, int reps
   out[gid] = acc;
 }
 
-// Round-2 design questions, measured for free by the round-end bench run (tba_microbench_ex):
+// Design questions, measured by every bench run before the timed solve (tba_microbench_ex):
 // k_red_rows: the element-major ("transposed", TBA_TRED) emission -- lanes 6q..6q+5 of a warp add to the 6 consecutive doubles
 // of one random 48-byte row (2 sectors), i.e. 32 elements cover ~11 sectors instead of 32.  G elements/s, comparable to k_red.
 __global__ void k_red_rows(double* y, unsigned n_rows, int reps) {
@@ -105,18 +105,17 @@ __global__ void k_gather_coop(const double* __restrict__ x, unsigned n_rows, int
   }
   out[gid] = acc;
 }
-// k_gather_256: rows padded to 64 bytes (8 doubles, 64-byte aligned): one 256-bit load (sm_100 LDG.E.ENL2.256) + one 128-bit load
-// per lane, 2 sectors of ONE 128-byte line per row.
-__global__ void k_gather_256(const double* __restrict__ x8, unsigned n_rows, int reps, double* out) {
+// k_gather_64: rows padded to 64 bytes (8 doubles, 64-byte aligned): three 128-bit loads per lane (sm_90 has no 256-bit load),
+// 2 sectors of ONE 128-byte line per row.
+__global__ void k_gather_64(const double* __restrict__ x8, unsigned n_rows, int reps, double* out) {
   const unsigned gid = blockIdx.x * blockDim.x + threadIdx.x;
   double acc = 0.0;
   for (int k = 0; k < reps; ++k) {
     const unsigned row = (gid * 2654435761u + (unsigned)k * 40503u) % n_rows;
     const double* p = x8 + (size_t)row * 8;
-    double a, b, c, d;
-    asm volatile("ld.global.nc.v4.f64 {%0,%1,%2,%3}, [%4];" : "=d"(a), "=d"(b), "=d"(c), "=d"(d) : "l"(p));
+    const double2 a = __ldg(reinterpret_cast<const double2*>(p)), b = __ldg(reinterpret_cast<const double2*>(p + 2));
     const double2 e = __ldg(reinterpret_cast<const double2*>(p + 4));
-    acc += a + b + c + d + e.x + e.y;
+    acc += a.x + a.y + b.x + b.y + e.x + e.y;
   }
   out[gid] = acc;
 }
@@ -147,7 +146,7 @@ extern "C" int tba_microbench(int device, double* out3) {
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || device < 0 || device >= ndev) return -5;
   if (cudaSetDevice(device) != cudaSuccess) return -3;
-  int sms = 148;
+  int sms = 132;
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
   const int blocks = sms * 16, threads = 256;
   const size_t nthreads = (size_t)blocks * threads;
@@ -182,13 +181,13 @@ extern "C" int tba_microbench(int device, double* out3) {
 
 // out[0] = element-major RED rate (k_red_rows), out[1] = shared-memory fp64 atomicAdd rate (k_smem_atomic),
 // out[2] = windowed global RED rate (k_red_win), all in G operations/s; out[3..5] = 48-byte row gather rates in G rows/s of
-// k_gather_coop / k_gather_256 / k_gather_elem (compare with tba_microbench's out[2]); best of 5 after a warm-up.  Diagnostics only.
+// k_gather_coop / k_gather_64 / k_gather_elem (compare with tba_microbench's out[2]); best of 5 after a warm-up.  Diagnostics only.
 extern "C" int tba_microbench_ex(int device, double* out6) {
   double* out3 = out6;
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || device < 0 || device >= ndev) return -5;
   if (cudaSetDevice(device) != cudaSuccess) return -3;
-  int sms = 148;
+  int sms = 132;
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
   const int blocks = sms * 16, threads = 256;
   const size_t nthreads = (size_t)blocks * threads;
@@ -206,7 +205,7 @@ extern "C" int tba_microbench_ex(int device, double* out6) {
   for (int rep = 0; rep < 6; ++rep) {
     cudaEventRecord(e0); k_gather_coop<<<blocks, threads>>>(d_y, n_y / 6, reps, d_out); cudaEventRecord(e1); cudaEventSynchronize(e1);
     const double g0 = time_ms(e0, e1) * 1e-3;
-    cudaEventRecord(e0); k_gather_256<<<blocks, threads>>>(d_x8, n_y / 6, reps, d_out); cudaEventRecord(e1); cudaEventSynchronize(e1);
+    cudaEventRecord(e0); k_gather_64<<<blocks, threads>>>(d_x8, n_y / 6, reps, d_out); cudaEventRecord(e1); cudaEventSynchronize(e1);
     const double g1 = time_ms(e0, e1) * 1e-3;
     cudaEventRecord(e0); k_gather_elem<<<blocks, threads>>>(d_y, n_y / 6, reps, d_out); cudaEventRecord(e1); cudaEventSynchronize(e1);
     const double g2 = time_ms(e0, e1) * 1e-3;
@@ -261,7 +260,7 @@ extern "C" int tba_microbench_gaps(int device, double* out5) {
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || device < 0 || device >= ndev) return -5;
   if (cudaSetDevice(device) != cudaSuccess) return -3;
-  int sms = 148;
+  int sms = 132;
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
   const int big_smem = 220 * 1024;
   if (cudaFuncSetAttribute(k_gap_big, cudaFuncAttributeMaxDynamicSharedMemorySize, big_smem) != cudaSuccess ||

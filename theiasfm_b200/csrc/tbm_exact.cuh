@@ -1,6 +1,6 @@
 // tbm_exact.cuh -- pass 2 of the tensor-core matcher (tbm_matcher_tc.cuh): the exact float re-evaluation of the candidates the TF32
 // pass selected, in the reference's summation order (distance.h:52-56), and the exhaustive scan of the queries whose candidate list
-// overflowed.  Plain CUDA (no tcgen05 / TMA): also compiled by the SIMT emulation build, where tbm_debug_exact_top2 drives it with
+// overflowed.  Plain CUDA (no wgmma / TMA): also compiled by the SIMT emulation build, where tbm_debug_exact_top2 drives it with
 // hand-made candidate lists (tests/test_matcher_host.py).
 #pragma once
 #include <cuda_runtime.h>
@@ -82,9 +82,8 @@ __device__ __forceinline__ void tile_store(float* s_rows, const float4 (&v)[kRow
 // Exhaustive scan of ONE query (row `a`, already in shared memory) against candidate rows [base, base + nb) by the whole CTA: tiles of
 // XT rows staged with coalesced loads, one row per thread 0 .. XT-1 in the reference's term order, then a top-2 merge of the XT
 // scanners.  All 256 threads must call it; m_* are [XT] scratch arrays.
-// (A register-staged, prefetching version of this loop and per-lane loads for the listed candidates were measured against this one on
-// the bench scene: 30.8 - 34.0 ms per step for all four combinations, i.e. no difference -- the scan is bound by its LSU wavefronts
-// (load + store + row read = 12 per row), not by load latency.  The plain loop stayed.)
+// (The scan is bound by its LSU wavefronts -- load + store + row read = 12 per row -- not by load latency: a register-staged,
+// prefetching version of this loop bought nothing, so the plain loop stayed.)
 __device__ __forceinline__ void exhaustive_scan(const float* __restrict__ d, const float* s_a, float* s_rows, int base, int nb, float* m_d,
                                                 float* m_d2, int* m_j, int* m_j2, int* out_j, float* out_d, float* out_d2) {
   const int tid = threadIdx.x;
@@ -109,6 +108,8 @@ __device__ __forceinline__ void exhaustive_scan(const float* __restrict__ d, con
   }
 }
 
+// k_nn_candidates marks an overflowed query in slot 0 only; slot KC / 2 is also honoured because it is part of the documented
+// input format of the tbm_debug_exact_top2 test hook (include/theia_matcher_b200.h), which callers use to build candidate lists.
 __device__ __forceinline__ bool list_overflowed(const int* __restrict__ cand, long long qi) {
   return cand[qi * KC] == kOverflow || cand[qi * KC + KC / 2] == kOverflow;
 }
@@ -116,7 +117,7 @@ __device__ __forceinline__ bool list_overflowed(const int* __restrict__ cand, lo
 constexpr int kExactSmemBytes = (XT + 32) * XS * (int)sizeof(float);  // dynamic shared memory: [XT] candidate rows + [32] query rows
 
 // One CTA = 32 queries, EVERY descriptor row goes through shared memory with coalesced loads.
-// Per-lane row loads (32 different rows per load instruction) made the first version of this pass LSU-bound (ncu: 93 % LSU wavefronts):
+// Per-lane row loads (32 different rows per load instruction) made the first version of this pass bound by its LSU wavefronts:
 //   * the 32 query rows are staged once;
 //   * the listed candidates of the 32 queries are compacted into ONE dense work list (ballot / popc per query, prefix over the queries)
 //     and evaluated XT rows per tile, one row per thread; a per-query thread then picks its two best from its slice of the list;

@@ -1,6 +1,6 @@
 // tbm_matcher.cu -- secondary path (SURVEY 8 row a16): brute-force descriptor matching on the GPU, C-ABI of
 // include/theia_matcher_b200.h.  Round-1 kernel: CUDA cores, exact float arithmetic in the reference's order (so the
-// match sets are bit-identical to the CPU restatement); NOT yet the tcgen05 distance GEMM (DESIGN.md section 8).
+// match sets are bit-identical to the CPU restatement); dim 128 takes the wgmma distance GEMM of tbm_matcher_tc.cuh.
 #include <cuda_runtime.h>
 
 #include <cstdint>
@@ -12,7 +12,7 @@
 #include "tbm_decide.cuh"       // MatchImagePair's decisions on the device (ratio test, early exits, IntersectMatches)
 #include "tbm_exact.cuh"        // exact re-evaluation of the tensor-core path's candidates (plain CUDA: in both builds)
 #ifndef TBA_EMULATE
-#include "tbm_matcher_tc.cuh"   // tcgen05 / TMA path (sm_100a); the SIMT emulation build keeps the exact CUDA-core kernels only
+#include "tbm_matcher_tc.cuh"   // wgmma / TMA path (sm_90a); the SIMT emulation build keeps the exact CUDA-core kernels only
 #endif
 #include <cstdlib>
 
@@ -259,7 +259,7 @@ static int match_all_tc(const float* descriptors, const int64_t* img_off, int32_
   struct EvGuard { cudaEvent_t* e; ~EvGuard() { for (int i = 0; i < 6; ++i) cudaEventDestroy(e[i]); } } ev_guard{ev};
   g_last_timing[0] = g_last_timing[1] = g_last_timing[2] = g_last_timing[3] = 0.0;
   cudaEventRecord(ev[0]);
-  int n_sm = 148;
+  int n_sm = 132;
   { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev); }
   DevF d_desc, d_nrm, d_bd, d_sd;
   DevI d_cand, d_bj, d_qrow, d_brow0, d_brows;

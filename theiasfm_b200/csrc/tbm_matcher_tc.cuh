@@ -1,4 +1,4 @@
-// tbm_matcher_tc.cuh -- tensor-core path of the brute-force matcher (SURVEY 8 row a16; sm_100a only).
+// tbm_matcher_tc.cuh -- tensor-core path of the brute-force matcher (SURVEY 8 row a16; sm_90a: wgmma + TMA + mbarrier).
 //
 // Replaces the hot loop of BruteForceFeatureMatcher::MatchImagePair
 // (src/theia/matching/brute_force_feature_matcher.cc:64-82 forward, :93-112 reverse; L2::operator() distance.h:52-56):
@@ -6,12 +6,12 @@
 //
 // Two passes per (image pair, direction):
 //   1. k_nn_candidates (this file): ||x - y||^2 = ||x||^2 + ||y||^2 - 2 x.y with the 128-dimensional dot products as a TF32
-//      tcgen05.mma GEMM -- a 128-query block of image A (resident in shared memory) against 128-candidate tiles of image B
-//      streamed by TMA (cp.async.bulk.tensor, 128-byte swizzle), fp32 accumulators double-buffered in TMEM -- and a fused
-//      epilogue that reads the accumulator tile back with tcgen05.ld and keeps, per query row, the candidates whose score
-//      ||y||^2 - 2 x.y lies within the TF32 error margin of the running runner-up (branch-free, lists in shared memory).
-//      Warp roles: 0 = TMA producer, 1 = MMA issuer (one elected lane) + TMEM allocation, 2..9 = epilogue (TMEM lane quarter
-//      warp % 4, column half (warp - 2) / 4).  Persistent CTAs over a list of work items.
+//      wgmma GEMM -- a 128-query block of image A (resident in shared memory) against 64-candidate tiles of image B streamed
+//      by TMA (cp.async.bulk.tensor, 128-byte swizzle, NSTAGE-deep ring) -- and a fused epilogue on the fp32 accumulator
+//      registers that keeps, per query row, the candidates whose score ||y||^2 - 2 x.y lies within the TF32 error margin of
+//      the running runner-up (branch-free, lists in shared memory).
+//      Warp roles: warpgroup 0 = TMA producer (one thread), warpgroups 1 and 2 = consumers: each issues the m64n64k8 wgmmas
+//      of its 64 query rows and scans its accumulators.  Persistent CTAs over a list of work items.
 //   2. k_exact_top2: the KC candidates of every query are re-evaluated EXACTLY -- float, term by term in the reference's
 //      order without fused multiply-add, like the round-1 kernel k_nn2 -- and the best two (ties: lower index) are kept.
 // TF32 only ranks candidates; every distance that leaves the GPU, every ratio test and every tie-break is computed from
@@ -23,20 +23,21 @@
 #include <cudaTypedefs.h>
 
 #include <cstdint>
-#include <cstdio>
 
 #include "tbm_exact.cuh"  // DIM, KC, ET, kOverflow + the exact re-evaluation kernel (plain CUDA, shared with the emulation build)
 
 namespace tbm_tc {
 
-constexpr int BM = 128;        // query rows per work item (= TMEM lanes)
-constexpr int BN = 128;        // candidate rows per tile (= accumulator columns)
-constexpr int CAP = 15;        // list slots per (query, column half) in shared memory: 12 usable (a list that reaches slot 11 => exact full scan of that query) + 3 spare behind them (pointer clamped once per four appends)
-constexpr int ATOM_BYTES = BM * 128;              // one 128-row x 128-byte swizzle-atom panel
-constexpr int TILE_BYTES = 4 * ATOM_BYTES;        // 64 KB: a 128 x 128 float tile
-constexpr int NSTAGE = 2;
-constexpr int EPI_WARPS = 8;                      // two per TMEM lane quarter: each scans one 64-column half of the tile
-constexpr int THREADS = 64 + 32 * EPI_WARPS;
+constexpr int BM = 128;        // query rows per work item (two consumer warpgroups x 64 rows)
+constexpr int BN = 64;         // candidate rows per tile (= accumulator columns of one m64n64 wgmma)
+constexpr int WG_ROWS = 64;    // query rows of one consumer warpgroup
+constexpr int CAP = 15;        // list slots per (query, column quarter) in shared memory: 11 usable (a list that reaches slot 11 => exact full scan of that query) + 4 spare behind them (pointer clamped once per four appends)
+constexpr int PANEL_BYTES = 64 * 128;             // one 64-row x 128-byte swizzle-atom panel (32 floats of 64 rows)
+constexpr int A_BYTES = 2 * 4 * PANEL_BYTES;      // 64 KB: the 128 x 128 float query block, [warpgroup][atom panel]
+constexpr int B_BYTES = 4 * PANEL_BYTES;          // 32 KB: a 64 x 128 float candidate tile
+constexpr int NSTAGE = 3;
+constexpr int THREADS = 3 * 128;
+constexpr int NLISTS = 2 * 256;                   // candidate lists: two query rows per consumer thread
 
 struct WorkItem {
   int a_row0;    // global row of the first query of this block
@@ -63,275 +64,272 @@ __device__ __forceinline__ bool bar_try(uint64_t* b, uint32_t parity) {
                : "=r"(ok) : "r"(smem_addr(b)), "r"(parity) : "memory");
   return ok != 0;
 }
+// (no printf on the timeout: a function call anywhere in the kernel makes ptxas serialise the wgmma pipeline)
 __device__ __forceinline__ void bar_wait(uint64_t* b, uint32_t parity) {
   if (bar_try(b, parity)) return;
   const long long t0 = clock64();
   while (!bar_try(b, parity)) {
-    if (clock64() - t0 > 4000000000ll) { printf("tbm: mbarrier wait timed out (block %d thread %d)\n", (int)blockIdx.x, (int)threadIdx.x); __trap(); }
+    if (clock64() - t0 > 4000000000ll) __trap();
   }
 }
 __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* map, int c0, int c1, uint64_t* bar) {
   asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
                ::"r"(smem_addr(dst)), "l"(map), "r"(smem_addr(bar)), "r"(c0), "r"(c1) : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_addr(bar)) : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]^T, both operands K-major, TF32 inputs, fp32 accumulation
-__device__ __forceinline__ void tc_mma_tf32(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-               ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
-// Shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): K-major operand, 128-byte swizzle, 8-row groups 1024 bytes apart.
+// Shared-memory matrix descriptor of wgmma (sm_90): K-major operand, 128-byte swizzle, 8-row groups 1024 bytes apart.
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);        // start address, 16-byte units
   d |= (uint64_t)1 << 16;                        // leading byte offset (unused with swizzled K-major layouts): 1
   d |= (uint64_t)(1024 >> 4) << 32;              // stride byte offset: 8 rows x 128 bytes
-  d |= (uint64_t)1 << 46;                        // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;                        // layout type SWIZZLE_128B
+  d |= (uint64_t)1 << 62;                        // layout type SWIZZLE_128B
   return d;
 }
-// Instruction descriptor (cute::UMMA::InstrDescriptor): D = F32, A = B = TF32, K-major both, N = 128, M = 128
-constexpr uint32_t kIdesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// D[64 x 64] (+)= A[smem, 64 x 8] * B[smem, 64 x 8]^T, both operands K-major, TF32 inputs, fp32 accumulation in registers
+__device__ __forceinline__ void wgmma_tf32(float (&d)[32], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, "
-      "%22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]),
-        "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]),
-        "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]),
+        "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]),
+        "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate)
       : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+}
+// keeps the compiler from moving accumulator reads above the wait of the asynchronous wgmma
+__device__ __forceinline__ void acc_fence(float (&d)[32]) {
+#pragma unroll
+  for (int i = 0; i < 32; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
 struct __align__(8) Ctl {
-  uint64_t a_full, a_empty, b_full[NSTAGE], b_empty[NSTAGE], acc_full[2], acc_empty[2];
-  uint32_t tmem_base;
+  uint64_t a_full, a_empty, b_full[NSTAGE], b_empty[NSTAGE];
 };
 
 // ------------------------------------------------------------------ pass 1: TF32 candidates
-// desc_map: the concatenated descriptor matrix [total_rows][128] float as a 2-D tensor map, box = 32 floats x 128 rows, SWIZZLE_128B.
-// nrm[r] = ||descriptor r||^2 (float).  cand[(out_row0 + m) * KC + k] = global row of the k-th best candidate of query m (-1: none).
+// desc_map: the concatenated descriptor matrix [total_rows][128] float as a 2-D tensor map, box = 32 floats x 64 rows, SWIZZLE_128B.
+// nrm[r] = ||descriptor r||^2 (float).  cand[(out_row0 + m) * KC + k] = global row of the k-th candidate of query m (-1: none).
 template <bool NONNEG>
 __global__ void __launch_bounds__(THREADS, 1) k_nn_candidates(const __grid_constant__ CUtensorMap desc_map, const WorkItem* __restrict__ items,
                                                               int n_items, const float* __restrict__ nrm, int* __restrict__ cand) {
   extern __shared__ uint8_t smem_raw[];
   // 128-byte-swizzled operand panels must start on 1024-byte boundaries (of the shared-memory address)
   uint8_t* smem = smem_raw + ((1024u - (smem_addr(smem_raw) & 1023u)) & 1023u);
-  uint8_t* sA = smem;                                  // 4 atom panels of the query block
-  uint8_t* sB = smem + TILE_BYTES;                     // NSTAGE x 4 atom panels of candidate tiles
-  float* sN = reinterpret_cast<float*>(smem + TILE_BYTES * (1 + NSTAGE));  // [2][BN] squared norms of the tile being drained
-  uint2* sC = reinterpret_cast<uint2*>(smem + TILE_BYTES * (1 + NSTAGE) + 2 * BN * sizeof(float));  // [CAP][256] provisional candidates (score bits, row)
-  Ctl* ctl = reinterpret_cast<Ctl*>(smem + TILE_BYTES * (1 + NSTAGE) + 2 * BN * sizeof(float) + (size_t)CAP * 2 * BM * sizeof(uint2));
+  uint8_t* sA = smem;                                  // [2 warpgroups][4 atom panels] of the query block
+  uint8_t* sB = smem + A_BYTES;                        // NSTAGE x 4 atom panels of candidate tiles
+  uint2* sC = reinterpret_cast<uint2*>(smem + A_BYTES + (size_t)NSTAGE * B_BYTES);  // [CAP][NLISTS] provisional candidates (score bits, row)
+  Ctl* ctl = reinterpret_cast<Ctl*>(smem + A_BYTES + (size_t)NSTAGE * B_BYTES + (size_t)CAP * NLISTS * sizeof(uint2));
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
-    bar_init(&ctl->a_full, 1); bar_init(&ctl->a_empty, 1);
-    for (int s = 0; s < NSTAGE; ++s) { bar_init(&ctl->b_full[s], 1); bar_init(&ctl->b_empty[s], 1); }
-    for (int a = 0; a < 2; ++a) { bar_init(&ctl->acc_full[a], 1); bar_init(&ctl->acc_empty[a], EPI_WARPS); }
+    bar_init(&ctl->a_full, 1); bar_init(&ctl->a_empty, 8);
+    for (int s = 0; s < NSTAGE; ++s) { bar_init(&ctl->b_full[s], 1); bar_init(&ctl->b_empty[s], 8); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {  // TMEM: 2 accumulators x 128 columns
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_addr(&ctl->tmem_base)), "n"(256) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = ctl->tmem_base;
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ===================== TMA producer =====================
-    if (lane == 0) {
+    if (threadIdx.x == 0) {
       uint32_t bt = 0, itc = 0;
       for (int it = blockIdx.x; it < n_items; it += gridDim.x, ++itc) {
         const WorkItem w = items[it];
-        bar_wait(&ctl->a_empty, (itc & 1) ^ 1);          // the MMAs of the previous item have read sA
-        bar_expect_tx(&ctl->a_full, TILE_BYTES);
-        for (int a = 0; a < 4; ++a) tma_load_2d(sA + a * ATOM_BYTES, &desc_map, a * 32, w.a_row0, &ctl->a_full);
+        bar_wait(&ctl->a_empty, (itc & 1) ^ 1);          // the wgmmas of the previous item have read sA
+        bar_expect_tx(&ctl->a_full, A_BYTES);
+        for (int g = 0; g < 2; ++g)
+          for (int a = 0; a < 4; ++a) tma_load_2d(sA + (g * 4 + a) * PANEL_BYTES, &desc_map, a * 32, w.a_row0 + g * WG_ROWS, &ctl->a_full);
         const int n_tiles = (w.b_rows + BN - 1) / BN;
         for (int t = 0; t < n_tiles; ++t, ++bt) {
           const int s = bt % NSTAGE;
           bar_wait(&ctl->b_empty[s], ((bt / NSTAGE) & 1) ^ 1);
-          bar_expect_tx(&ctl->b_full[s], TILE_BYTES);
-          for (int a = 0; a < 4; ++a) tma_load_2d(sB + (size_t)s * TILE_BYTES + a * ATOM_BYTES, &desc_map, a * 32, w.b_row0 + t * BN, &ctl->b_full[s]);
+          bar_expect_tx(&ctl->b_full[s], B_BYTES);
+          for (int a = 0; a < 4; ++a) tma_load_2d(sB + (size_t)s * B_BYTES + a * PANEL_BYTES, &desc_map, a * 32, w.b_row0 + t * BN, &ctl->b_full[s]);
         }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      uint32_t bt = 0, itc = 0;
-      for (int it = blockIdx.x; it < n_items; it += gridDim.x, ++itc) {
-        const WorkItem w = items[it];
-        bar_wait(&ctl->a_full, itc & 1);
-        const int n_tiles = (w.b_rows + BN - 1) / BN;
-        for (int t = 0; t < n_tiles; ++t, ++bt) {
-          const int s = bt % NSTAGE, acc = bt & 1;
-          bar_wait(&ctl->b_full[s], (bt / NSTAGE) & 1);
-          bar_wait(&ctl->acc_empty[acc], ((bt >> 1) & 1) ^ 1);   // the epilogue has drained this accumulator
-          tc_fence_after();
-          const uint32_t a0 = smem_addr(sA), b0 = smem_addr(sB + (size_t)s * TILE_BYTES);
-#pragma unroll
-          for (int a = 0; a < 4; ++a)
-#pragma unroll
-            for (int k = 0; k < 4; ++k)  // UMMA_K = 8 tf32 = 32 bytes inside the 128-byte swizzle atom
-              tc_mma_tf32(tmem + acc * BN, make_desc(a0 + a * ATOM_BYTES + k * 32), make_desc(b0 + a * ATOM_BYTES + k * 32), kIdesc, (a | k) != 0);
-          tc_commit(&ctl->b_empty[s]);      // the stage can be refilled once these MMAs have read it
-          tc_commit(&ctl->acc_full[acc]);   // ... and the accumulator is complete
-        }
-        tc_commit(&ctl->a_empty);
       }
     }
   } else {
-    // ===================== epilogue: 8 warps = 4 TMEM lane quarters (warp % 4) x 2 column halves =====================
-    // Branch-free streaming selection.  A thread owns one query row and one 64-column half of every candidate tile; it keeps the
-    // running two smallest scores m1 <= m2 of  score(n) = ||y_n||^2 - 2 x.y_n  over ITS columns (three min/max per element) and
-    // appends an element to its candidate list in shared memory -- one predicated 8-byte store, no branch, no divergence -- whenever
+    // ===================== consumers: wgmma + epilogue on the accumulator registers =====================
+    // Accumulator layout of m64n64 (per warp w of the warpgroup, lane l): d[4j + 2i + c] = row 16w + l/4 + 8i, column 8j + 2(l%4) + c.
+    // A thread therefore owns two query rows (i = 0, 1) and one column quarter (l % 4) of each: 16 of the 64 columns of every tile.
+    //
+    // Branch-free streaming selection.  Per (row, quarter) the thread keeps the running two smallest scores m1 <= m2 of
+    // score(n) = ||y_n||^2 - 2 x.y_n over ITS columns (three min/max per element) and appends an element to its candidate list in
+    // shared memory -- one predicated 8-byte store, no branch, no divergence -- whenever
     //     score(n) < m2 + margin(n),
-    // where margin(n) is at least twice the worst-case TF32 error of a score.  tcgen05 kind::tf32 uses 10 mantissa bits of each
-    // operand (relative operand error < 2^-10 truncating, <= 2^-11 rounding), so |d score| <= 2 * 2^-9 sum_k |x_k y_k|:
+    // where margin(n) is at least twice the worst-case TF32 error of a score.  wgmma .tf32 uses 10 mantissa bits of each operand
+    // (relative operand error < 2^-10 truncating, <= 2^-11 rounding), so |d score| <= 2 * 2^-9 sum_k |x_k y_k|:
     //   * NONNEG (every descriptor component >= 0: SIFT, RootSIFT, any histogram descriptor): sum_k |x_k y_k| = x.y, read off the
     //     accumulator itself: margin(n) = 2^-8 x.y_n (1 + 2^-6)  (truncation errors are one-sided there, so 1 x the bound suffices;
     //     with rounding the bound halves and 2 x it is the same number);
     //   * otherwise: sum_k |x_k y_k| <= ||x|| ||y|| <= (||x||^2 + ||y||^2) / 2:  margin(n) = 2^-8 (||x||^2 + ||y_n||^2).
-    // An element that is among the two nearest of the whole image in
-    // exact arithmetic is a fortiori among the two nearest of its half: it passes the test when it is seen (m2 only decreases) and
-    // stays below every later m2 + margin, so it survives the compactions (a list that grows past 8 drops the entries above the
-    // current limit) and reaches the exact pass, which re-evaluates the union of the two halves' lists.  A list that fills up
-    // (a dense cluster of near-identical candidates) flags the row: the exact pass then scans every candidate of that query.
+    // An element that is among the two nearest of the whole image in exact arithmetic is a fortiori among the two nearest of its
+    // quarter: it passes the test when it is seen (m2 only decreases) and stays below every later m2 + margin, so it survives the
+    // compactions (a list that grows past 8 drops the entries above the current limit).  At the end of an item the four quarters of
+    // a row merge their (m1, m2) by shuffles; the entries within the margin of the row's own runner-up -- the same test on the whole
+    // row -- are written to the KC slots of the query for the exact pass.  A list that fills up, or a row with more than KC such
+    // entries (a dense cluster of near-identical candidates), flags the row: the exact pass then scans every candidate of that query.
     // The first tile is scanned twice: once only to establish m1, m2 (otherwise every element of it would be appended).
-    const int q = warp & 3;                 // TMEM lane quarter of this warp
-    const int half = (warp - 2) >> 2;       // column half: warps 2..5 -> 0, warps 6..9 -> 1
-    const int row = q * 32 + lane;          // query row of this thread inside the block
-    const int et = threadIdx.x - 64;        // 0..255 among the epilogue threads
+    const int g = warp / 4 - 1;              // consumer warpgroup: query rows [64 g, 64 g + 64) of the block
+    const int wl = warp & 3;
+    const int et = threadIdx.x - 128;        // 0..255 among the consumer threads
+    const int cq = lane & 3;                 // column quarter
     const float kInf = __int_as_float(0x7f800000);
-    uint2* myC = sC + et;                   // list entries of this thread: myC[k * 2 * BM]
-    constexpr uint32_t kStride = 2 * BM * (uint32_t)sizeof(uint2);   // bytes between consecutive entries of one list
-    const uint32_t c_base = smem_addr(myC), c_last = c_base + (CAP - 4) * kStride;
-    uint32_t bt = 0;
-    for (int it = blockIdx.x; it < n_items; it += gridDim.x) {
+    constexpr uint32_t kStride = NLISTS * (uint32_t)sizeof(uint2);   // bytes between consecutive entries of one list
+    const uint32_t a_base = smem_addr(sA + g * 4 * PANEL_BYTES);
+    float acc[32];
+#pragma unroll
+    for (int k = 0; k < 32; ++k) acc[k] = 0.0f;
+    uint32_t bt = 0, itc = 0;
+    for (int it = blockIdx.x; it < n_items; it += gridDim.x, ++itc) {
       const WorkItem w = items[it];
-      float m1 = kInf, m2 = kInf;
-      const float nx8 = (!NONNEG && row < w.a_rows) ? 0.00390625f * __ldg(nrm + w.a_row0 + row) : 0.0f;  // 2^-8 ||x||^2 (general margin only)
-      // wp = shared-memory address of the next append; it saturates at the last slot, and a list that reaches the last slot
-      // counts as overflowed (capacity CAP - 4 entries between two maintenance points)
-      uint32_t wp = c_base;
-      int ovf = 0;
+      int row[2];
+      float m1[2], m2[2], nx8[2];
+      uint32_t c_base[2], c_last[2], wp[2];
+      int ovf[2];
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        row[i] = g * WG_ROWS + wl * 16 + (lane >> 2) + 8 * i;   // query row of this thread inside the block
+        m1[i] = kInf; m2[i] = kInf;
+        nx8[i] = (!NONNEG && row[i] < w.a_rows) ? 0.00390625f * __ldg(nrm + w.a_row0 + row[i]) : 0.0f;  // 2^-8 ||x||^2 (general margin only)
+        // wp = shared-memory address of the next append; it saturates at the last slot, and a list that reaches the last slot
+        // counts as overflowed (capacity CAP - 4 entries between two maintenance points)
+        c_base[i] = smem_addr(sC + i * 256 + et);
+        c_last[i] = c_base[i] + (CAP - 4) * kStride;
+        wp[i] = c_base[i];
+        ovf[i] = 0;
+      }
+      bar_wait(&ctl->a_full, itc & 1);
       const int n_tiles = (w.b_rows + BN - 1) / BN;
       for (int t = 0; t < n_tiles; ++t, ++bt) {
-        const int acc = bt & 1;
-        // squared norms of this tile's candidates, double-buffered in shared memory
-        if (et < BN) {
-          const int col_row = t * BN + et;
-          sN[acc * BN + et] = col_row < w.b_rows ? __ldg(nrm + w.b_row0 + col_row) : kInf;
+        const int s = bt % NSTAGE;
+        bar_wait(&ctl->b_full[s], (bt / NSTAGE) & 1);
+        __syncwarp();   // wgmma is .sync.aligned: the warp must be converged after the spin of the wait
+        const uint32_t b_base = smem_addr(sB + (size_t)s * B_BYTES);
+        wg_fence();
+#pragma unroll
+        for (int a = 0; a < 4; ++a)
+#pragma unroll
+          for (int k = 0; k < 4; ++k)  // K = 8 tf32 = 32 bytes inside the 128-byte swizzle atom
+            wgmma_tf32(acc, make_desc(a_base + a * PANEL_BYTES + k * 32), make_desc(b_base + a * PANEL_BYTES + k * 32), (a | k) != 0);
+        wg_commit();
+        // squared norms of this thread's 16 columns of the tile, loaded while the wgmmas run
+        float nn[8][2];
+        const int jt = t * BN + 2 * cq;
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+#pragma unroll
+          for (int c = 0; c < 2; ++c) nn[j][c] = jt + 8 * j + c < w.b_rows ? __ldg(nrm + w.b_row0 + jt + 8 * j + c) : kInf;
+        wg_wait0();
+        acc_fence(acc);
+        __syncwarp();
+        if (lane == 0) {
+          bar_arrive(&ctl->b_empty[s]);                   // this warp's wgmmas have read the stage
+          if (t == n_tiles - 1) bar_arrive(&ctl->a_empty);  // ... and the query block
         }
-        asm volatile("bar.sync 1, 256;" ::: "memory");  // the eight epilogue warps
-        bar_wait(&ctl->acc_full[acc], (bt >> 1) & 1);
-        tc_fence_after();
-        const uint32_t taddr = tmem + ((uint32_t)(q * 32) << 16) + acc * BN + half * 64;
-        const float4* nt4 = reinterpret_cast<const float4*>(sN + acc * BN + half * 64);
-        const int jt = w.b_row0 + t * BN + half * 64;
+        const int jg = w.b_row0 + jt;   // global row of column (j = 0, c = 0)
         // one predicated 8-byte store + pointer bump per element; the pointer is clamped to the last slot once per FOUR elements
         // (TBM_CLAMP): at most four appends can happen in between, and the lists keep four spare slots behind c_last for them
-#define TBM_APPEND(VAL, J)                                                                                              \
+#define TBM_APPEND(I, VAL, J)                                                                                           \
   asm volatile("{\n\t.reg .pred p;\n\tsetp.lt.f32 p, %1, %2;\n\t@p st.shared.v2.b32 [%0], {%3, %4};\n\t@p add.u32 %0, %0, %5;\n\t}"      \
-               : "+r"(wp) : "f"(VAL), "f"(lim), "r"(__float_as_uint(VAL)), "r"(J), "n"(kStride) : "memory")
-#define TBM_CLAMP() wp = min(wp, c_last)
-        if (t == 0) {
-#pragma unroll 1
-          for (int c0 = 0; c0 < 64; c0 += 32) {
-            uint32_t r[32];
-            tmem_ld32(taddr + c0, r);
+               : "+r"(wp[I]) : "f"(VAL), "f"(lim), "r"(__float_as_uint(VAL)), "r"(J), "n"(kStride) : "memory")
+#define TBM_CLAMP(I) wp[I] = min(wp[I], c_last[I])
 #pragma unroll
-            for (int c4 = 0; c4 < 8; ++c4) {
-              const float4 n4 = nt4[(c0 >> 2) + c4];
-              const float nn[4] = {n4.x, n4.y, n4.z, n4.w};
+        for (int i = 0; i < 2; ++i) {
+          if (t == 0) {  // tile 0: m1, m2 first, then the appends against them (counting an element twice would turn the best into its own runner-up)
 #pragma unroll
-              for (int u = 0; u < 4; ++u) {
-                const float sc = fmaf(-2.0f, __uint_as_float(r[4 * c4 + u]), nn[u]);
-                m2 = fminf(m2, fmaxf(m1, sc));
-                m1 = fminf(m1, sc);
+            for (int j = 0; j < 8; ++j)
+#pragma unroll
+              for (int c = 0; c < 2; ++c) {
+                const float sc = fmaf(-2.0f, acc[4 * j + 2 * i + c], nn[j][c]);
+                m2[i] = fminf(m2[i], fmaxf(m1[i], sc));
+                m1[i] = fminf(m1[i], sc);
               }
-            }
-          }
-        }
-#pragma unroll 1
-        for (int c0 = 0; c0 < 64; c0 += 32) {
-          uint32_t r[32];
-          tmem_ld32(taddr + c0, r);
-          if (t == 0) {  // (tile 0 is already in m1, m2: counting an element twice would turn the best into its own runner-up)
-            const float lim = NONNEG ? m2 : m2 + nx8;
+            const float lim = NONNEG ? m2[i] : m2[i] + nx8[i];
 #pragma unroll
-            for (int c4 = 0; c4 < 8; ++c4) {
-              const float4 n4 = nt4[(c0 >> 2) + c4];
-              const float nn[4] = {n4.x, n4.y, n4.z, n4.w};
+            for (int j = 0; j < 8; ++j) {
 #pragma unroll
-              for (int u = 0; u < 4; ++u) {
-                const float dotv = __uint_as_float(r[4 * c4 + u]);
-                const float val = fmaf(NONNEG ? dotv : nn[u], NONNEG ? -0.00396728515625f : -0.00390625f, fmaf(-2.0f, dotv, nn[u]));
-                TBM_APPEND(val, jt + c0 + 4 * c4 + u);
+              for (int c = 0; c < 2; ++c) {
+                const float dotv = acc[4 * j + 2 * i + c];
+                const float val = fmaf(NONNEG ? dotv : nn[j][c], NONNEG ? -0.00396728515625f : -0.00390625f, fmaf(-2.0f, dotv, nn[j][c]));
+                TBM_APPEND(i, val, jg + 8 * j + c);
               }
-              TBM_CLAMP();
+              if (j & 1) TBM_CLAMP(i);
             }
           } else {
 #pragma unroll
-            for (int c4 = 0; c4 < 8; ++c4) {
-              const float4 n4 = nt4[(c0 >> 2) + c4];
-              const float nn[4] = {n4.x, n4.y, n4.z, n4.w};
+            for (int j = 0; j < 8; ++j) {
 #pragma unroll
-              for (int u = 0; u < 4; ++u) {
-                const float dotv = __uint_as_float(r[4 * c4 + u]);
-                const float sc = fmaf(-2.0f, dotv, nn[u]);
-                const float val = fmaf(NONNEG ? dotv : nn[u], NONNEG ? -0.00396728515625f : -0.00390625f, sc);   // score minus the candidate's margin
-                const float lim = NONNEG ? m2 : m2 + nx8;
-                TBM_APPEND(val, jt + c0 + 4 * c4 + u);
-                m2 = fminf(m2, fmaxf(m1, sc));
-                m1 = fminf(m1, sc);
+              for (int c = 0; c < 2; ++c) {
+                const float dotv = acc[4 * j + 2 * i + c];
+                const float sc = fmaf(-2.0f, dotv, nn[j][c]);
+                const float val = fmaf(NONNEG ? dotv : nn[j][c], NONNEG ? -0.00396728515625f : -0.00390625f, sc);   // score minus the candidate's margin
+                const float lim = NONNEG ? m2[i] : m2[i] + nx8[i];
+                TBM_APPEND(i, val, jg + 8 * j + c);
+                m2[i] = fminf(m2[i], fmaxf(m1[i], sc));
+                m1[i] = fminf(m1[i], sc);
               }
-              TBM_CLAMP();
+              if (j & 1) TBM_CLAMP(i);
             }
           }
-#undef TBM_APPEND
-#undef TBM_CLAMP
-          // list maintenance, once per 32-column chunk (rare per lane; divergent, but cheap)
-          ovf |= wp == c_last;
-          if (wp > c_base + 8 * kStride) {
-            const int cnt = (int)((wp - c_base) / kStride);
-            const float lim = m2 + nx8;
+          // list maintenance, once per tile (rare per lane; divergent, but cheap)
+          ovf[i] |= wp[i] == c_last[i];
+          if (wp[i] > c_base[i] + 8 * kStride) {
+            const int cnt = (int)((wp[i] - c_base[i]) / kStride);
+            const float lim = m2[i] + nx8[i];
+            uint2* myC = sC + i * 256 + et;
             int k = 0;
             for (int e = 0; e < cnt; ++e) {
-              const uint2 ce = myC[e * 2 * BM];
-              if (__uint_as_float(ce.x) < lim) { myC[k * 2 * BM] = ce; ++k; }
+              const uint2 ce = myC[e * NLISTS];
+              if (__uint_as_float(ce.x) < lim) { myC[k * NLISTS] = ce; ++k; }
             }
-            wp = c_base + (uint32_t)k * kStride;
+            wp[i] = c_base[i] + (uint32_t)k * kStride;
           }
         }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) bar_arrive(&ctl->acc_empty[acc]);
+#undef TBM_APPEND
+#undef TBM_CLAMP
       }
-      const int cnt = (int)((wp - c_base) / kStride);
-      if (row < w.a_rows) {
-        int* o = cand + (size_t)(w.out_row0 + row) * KC + half * (KC / 2);   // slots [0, 8): columns half 0, [8, 16): half 1
-        const float lim = m2 + nx8;   // the final runner-up of this half: only entries within its margin can matter
-        int k = 0;
-        for (int e = 0; e < cnt; ++e) {
-          const uint2 ce = myC[e * 2 * BM];
-          if (__uint_as_float(ce.x) < lim) { if (k < KC / 2) o[k] = (int)ce.y; ++k; }
+      // ---- the row's runner-up over its four quarters (lanes 4r .. 4r + 3), then the kept entries into the KC slots of the query
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        float r1 = m1[i], r2 = m2[i];
+#pragma unroll
+        for (int o = 1; o <= 2; o <<= 1) {
+          const float o1 = __shfl_xor_sync(0xffffffffu, r1, o), o2 = __shfl_xor_sync(0xffffffffu, r2, o);
+          r2 = fminf(fmaxf(r1, o1), fminf(r2, o2));
+          r1 = fminf(r1, o1);
         }
-        if (ovf || k > KC / 2) o[0] = kOverflow;
-        else for (; k < KC / 2; ++k) o[k] = -1;
+        const float lim = r2 + nx8[i];   // the final runner-up of the row: only entries within its margin can matter
+        const uint2* myC = sC + i * 256 + et;
+        const int cnt = (int)((wp[i] - c_base[i]) / kStride);
+        int k = 0;
+        for (int e = 0; e < cnt; ++e) k += __uint_as_float(myC[e * NLISTS].x) < lim;
+        int before = 0, total = 0, any_ovf = 0;
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const int kq = __shfl_sync(0xffffffffu, k, (lane & ~3) | q);
+          total += kq;
+          before += q < cq ? kq : 0;
+          any_ovf |= __shfl_sync(0xffffffffu, ovf[i], (lane & ~3) | q);
+        }
+        if (row[i] < w.a_rows) {
+          int* o = cand + (size_t)(w.out_row0 + row[i]) * KC;
+          if (any_ovf || total > KC) {
+            if (cq == 0) o[0] = kOverflow;
+          } else {
+            int n = before;
+            for (int e = 0; e < cnt; ++e) {
+              const uint2 ce = myC[e * NLISTS];
+              if (__uint_as_float(ce.x) < lim) o[n++] = (int)ce.y;
+            }
+            if (cq == 3) for (int q = total; q < KC; ++q) o[q] = -1;
+          }
+        }
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "n"(256) : "memory");
 }
 
 // ||d||^2 of every descriptor row (float, plain left-to-right sum: only used to RANK candidates); *any_negative is set when a
@@ -362,12 +360,14 @@ inline bool make_desc_map(CUtensorMap* map, const float* d_desc, long long n_row
   }
   const cuuint64_t dims[2] = {(cuuint64_t)DIM, (cuuint64_t)n_rows};
   const cuuint64_t strides[1] = {(cuuint64_t)DIM * sizeof(float)};
-  const cuuint32_t box[2] = {32u, (cuuint32_t)BM};
+  const cuuint32_t box[2] = {32u, (cuuint32_t)BN};
   const cuuint32_t estr[2] = {1u, 1u};
   return encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(d_desc), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                 CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-constexpr size_t kSmemBytes = (size_t)TILE_BYTES * (1 + NSTAGE) + 2 * BN * sizeof(float) + (size_t)CAP * 2 * BM * sizeof(uint2) + sizeof(Ctl) + 1024;
+constexpr size_t kSmemBytes = (size_t)A_BYTES + (size_t)NSTAGE * B_BYTES + (size_t)CAP * NLISTS * sizeof(uint2) + sizeof(Ctl) + 1024;
+static_assert(kSmemBytes <= 227 * 1024, "k_nn_candidates must fit the 227 KB of shared memory an H100 block can have");
+static_assert(BN == WG_ROWS, "one tensor map (box 32 floats x 64 rows) serves both operands");
 
 }  // namespace tbm_tc

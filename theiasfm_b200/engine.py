@@ -1,6 +1,6 @@
 """ctypes binding of the C-ABI (include/theia_ba_b200.h) -> theiasfm_b200/libtheia_ba_b200.so.
 
-There is NO CPU fallback: if the CUDA library is missing, or no B200 is visible, construction
+There is NO CPU fallback: if the CUDA library is missing, or no CUDA device is visible, construction
 of an ``Engine`` raises.  The product path never touches ``oracle/``.
 """
 import ctypes as C
