@@ -63,6 +63,14 @@ void tbm_debug_last_timing(double* out4);
 int tbm_debug_exact_top2(int device, const float* descriptors, int64_t n_rows, const int32_t* q_row, const int32_t* b_row0,
                          const int32_t* b_rows, const int32_t* cand, int64_t n_q, int32_t* best_j, float* best_d, float* second_d);
 
+/* Test hook: the nearest-neighbour stage of tbm_match_all alone (same inputs and path: the tensor-core path for dim 128 unless
+ * TBM_PATH=exact), i.e. the per-query results the decision stage consumes.  For every pair, in pair order: its n1 forward queries,
+ * then, when symmetric != 0, its n2 reverse queries.  best_j = nearest candidate (-1: the other image is empty), best_d / second_d =
+ * exact float distances of the nearest and second-nearest (0 when missing); exhaustive[q] = 1 when the tensor-core candidate pass
+ * handed query q to the exhaustive exact scan (always 0 on the CUDA-core path).  Returns 0 or a tbm_match_all error code. */
+int tbm_debug_nn2(int device, const float* descriptors, const int64_t* img_off, int32_t n_img, int32_t dim, const int32_t* pairs,
+                  int64_t n_pairs, int symmetric, int32_t* best_j, float* best_d, float* second_d, uint8_t* exhaustive);
+
 #ifdef __cplusplus
 }
 #endif

@@ -108,6 +108,12 @@ using DevI = Dev<int>;
 
 static_assert(sizeof(tbm_match) == 12, "k_gather_matches copies a match as three 32-bit words");
 
+// Per-query results of the nearest-neighbour stage (what k_pair_decide consumes), copied to the host after every chunk / pair for
+// tbm_debug_nn2; layout per pair: forward queries [n1], then reverse queries [n2] when matching is symmetric.  nullptr: normal call.
+struct Nn2Out {
+  int32_t* best_j; float* best_d; float* second_d; uint8_t* exhaustive;
+};
+
 // Device buffers of the decision stage, kept for the whole call (grown on demand).
 struct DecideBuffers {
   Dev<tbm::PairSeg> segs;
@@ -250,7 +256,7 @@ int tbm_debug_postprocess(const int32_t* f_best_j, const float* f_best_d, const 
 // Tensor-core path (dim == 128): all pairs of a chunk in ONE launch of k_nn_candidates + ONE launch of k_exact_top2, one
 // device-to-host copy per chunk, then MatchImagePair's ratio test / early exits / IntersectMatches per pair on the host.
 static int match_all_tc(const float* descriptors, const int64_t* img_off, int32_t n_img, const int32_t* pairs, int64_t n_pairs,
-                        const tbm_options* options, tbm_match* matches, int64_t cap, int64_t* match_off, uint8_t* pair_ok) {
+                        const tbm_options* options, tbm_match* matches, int64_t cap, int64_t* match_off, uint8_t* pair_ok, const Nn2Out* dbg) {
   using namespace tbm_tc;
   const int64_t total = img_off[n_img];
   if (total >= (int64_t)1 << 31) return -1;
@@ -292,6 +298,7 @@ static int match_all_tc(const float* descriptors, const int64_t* img_off, int32_
   int64_t written = 0;
   bool overflow = false;
   const int64_t kChunkQueries = (int64_t)4 << 20;  // queries per chunk (both directions): bounds the device staging
+  int64_t q_base = 0;                                // queries of the chunks before this one (tbm_debug_nn2 output offset)
   for (int64_t p0 = 0; p0 < n_pairs;) {
     // ---- chunk [p0, p1): as many pairs as fit the query budget; one (pair, direction) segment table instead of per-query host arrays
     items.clear(); qsegs.clear(); psegs.clear();
@@ -344,7 +351,16 @@ static int match_all_tc(const float* descriptors, const int64_t* img_off, int32_
       cudaEventRecord(ev[4]);
       if (launch_exact_top2(d_desc.p, d_qrow.p, d_brow0.p, d_brows.p, d_cand.p, nq_chunk, d_bj.p, d_bd.p, d_sd.p, d_nex) != 0) return -3;
       cudaEventRecord(ev[5]);
+      if (dbg) {
+        std::vector<int> slot0((size_t)nq_chunk);  // candidate slot 0 of every query: kOverflow = scanned exhaustively
+        if (cudaMemcpy(dbg->best_j + q_base, d_bj.p, (size_t)nq_chunk * sizeof(int), cudaMemcpyDeviceToHost) != cudaSuccess ||
+            cudaMemcpy(dbg->best_d + q_base, d_bd.p, (size_t)nq_chunk * sizeof(float), cudaMemcpyDeviceToHost) != cudaSuccess ||
+            cudaMemcpy(dbg->second_d + q_base, d_sd.p, (size_t)nq_chunk * sizeof(float), cudaMemcpyDeviceToHost) != cudaSuccess ||
+            cudaMemcpy2D(slot0.data(), sizeof(int), d_cand.p, KC * sizeof(int), sizeof(int), (size_t)nq_chunk, cudaMemcpyDeviceToHost) != cudaSuccess) return -3;
+        for (int64_t q = 0; q < nq_chunk; ++q) dbg->exhaustive[q_base + q] = slot0[(size_t)q] == kOverflow;
+      }
     }
+    q_base += nq_chunk;
     // ---- MatchImagePair's decisions per pair, on the device (tbm_decide.cuh); only the kept matches are copied back
     const int rc = decide_and_fetch(dec, psegs, nq_chunk, d_bj.p, d_bd.p, d_sd.p, options, p0, matches, cap, &written, match_off, pair_ok, &overflow);
     if (rc) return rc;
@@ -364,8 +380,9 @@ static int match_all_tc(const float* descriptors, const int64_t* img_off, int32_
 }
 #endif
 
-int tbm_match_all(int device, const float* descriptors, const int64_t* img_off, int32_t n_img, int32_t dim, const int32_t* pairs,
-                  int64_t n_pairs, const tbm_options* options, tbm_match* matches, int64_t cap, int64_t* match_off, uint8_t* pair_ok) {
+static int match_all(int device, const float* descriptors, const int64_t* img_off, int32_t n_img, int32_t dim, const int32_t* pairs,
+                     int64_t n_pairs, const tbm_options* options, tbm_match* matches, int64_t cap, int64_t* match_off, uint8_t* pair_ok,
+                     const Nn2Out* dbg) {
   if (!descriptors || !img_off || !pairs || !options || !match_off || !pair_ok || n_img < 0 || dim <= 0 || dim > 512 || n_pairs < 0) return -1;
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev <= 0 || device < 0 || device >= ndev) { cudaGetLastError(); return -5; }
@@ -375,7 +392,7 @@ int tbm_match_all(int device, const float* descriptors, const int64_t* img_off, 
     // dim 128 (SIFT): the tensor-core path.  TBM_PATH=exact forces the CUDA-core kernel (the bit-exact checker of round 1).
     const char* e = getenv("TBM_PATH");
     for (int i = 0; i < n_img; ++i) if (img_off[i + 1] < img_off[i]) return -1;
-    if (dim == tbm_tc::DIM && !(e != nullptr && e[0] == 'e')) return match_all_tc(descriptors, img_off, n_img, pairs, n_pairs, options, matches, cap, match_off, pair_ok);
+    if (dim == tbm_tc::DIM && !(e != nullptr && e[0] == 'e')) return match_all_tc(descriptors, img_off, n_img, pairs, n_pairs, options, matches, cap, match_off, pair_ok, dbg);
   }
 #endif
   const int64_t total = img_off[n_img];
@@ -387,12 +404,14 @@ int tbm_match_all(int device, const float* descriptors, const int64_t* img_off, 
   if (!d_bd.alloc((size_t)max_n * 2) || !d_sd.alloc((size_t)max_n * 2) || !d_bj.alloc((size_t)max_n * 2)) return -3;
   if (cudaMemcpy(d_desc.p, descriptors, (size_t)total * dim * sizeof(float), cudaMemcpyHostToDevice) != cudaSuccess) return -3;
   const size_t smem = ((size_t)ROWS * (dim + 1) + (size_t)TJ * dim) * sizeof(float);
-  if (smem > 48 * 1024 && cudaFuncSetAttribute(k_nn2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return -3;
+  // the 48 KB a launch may use without the attribute include k_nn2's static s_merge (4 KB): dims 176..191 need it as well
+  if (cudaFuncSetAttribute(k_nn2, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return -3;
   DecideBuffers dec;
   std::vector<tbm::PairSeg> one(1);
   int64_t written = 0;
   bool overflow = false;
   const bool sym = options->keep_only_symmetric_matches != 0;
+  int64_t q_base = 0;  // tbm_debug_nn2 output offset of the current pair
   for (int64_t p = 0; p < n_pairs; ++p) {
     const int a = pairs[2 * p], b = pairs[2 * p + 1];
     if (a < 0 || a >= n_img || b < 0 || b >= n_img) return -1;
@@ -400,6 +419,8 @@ int tbm_match_all(int device, const float* descriptors, const int64_t* img_off, 
     const float* A = d_desc.p + (size_t)img_off[a] * dim;
     const float* B = d_desc.p + (size_t)img_off[b] * dim;
     if (n1 + n2 > 0 && cudaMemset(d_bj.p, 0xFF, (size_t)(n1 + n2) * sizeof(int)) != cudaSuccess) return -3;  // -1: no match (empty other image)
+    if (dbg && n1 + n2 > 0 && (cudaMemset(d_bd.p, 0, (size_t)(n1 + n2) * sizeof(float)) != cudaSuccess ||
+                               cudaMemset(d_sd.p, 0, (size_t)(n1 + n2) * sizeof(float)) != cudaSuccess)) return -3;
     for (int dir = 0; dir < (sym ? 2 : 1); ++dir) {
       const int nq = dir == 0 ? n1 : n2, nc = dir == 0 ? n2 : n1;
       if (nq == 0 || nc == 0) continue;
@@ -410,9 +431,43 @@ int tbm_match_all(int device, const float* descriptors, const int64_t* img_off, 
     one[0].f0 = 0; one[0].r0 = n1; one[0].n1 = n1; one[0].n2 = n2; one[0].n_rev = sym ? n2 : 0;
     const int rc = decide_and_fetch(dec, one, (long long)n1 + n2, d_bj.p, d_bd.p, d_sd.p, options, p, matches, cap, &written, match_off, pair_ok, &overflow);
     if (rc) return rc;
+    if (dbg) {
+      const size_t nq = (size_t)n1 + (sym ? (size_t)n2 : 0);
+      if (nq > 0 && (cudaMemcpy(dbg->best_j + q_base, d_bj.p, nq * sizeof(int), cudaMemcpyDeviceToHost) != cudaSuccess ||
+                     cudaMemcpy(dbg->best_d + q_base, d_bd.p, nq * sizeof(float), cudaMemcpyDeviceToHost) != cudaSuccess ||
+                     cudaMemcpy(dbg->second_d + q_base, d_sd.p, nq * sizeof(float), cudaMemcpyDeviceToHost) != cudaSuccess)) return -3;
+      q_base += (int64_t)nq;
+    }
   }
   match_off[n_pairs] = written;
   return overflow ? -1 : 0;
+}
+
+int tbm_match_all(int device, const float* descriptors, const int64_t* img_off, int32_t n_img, int32_t dim, const int32_t* pairs,
+                  int64_t n_pairs, const tbm_options* options, tbm_match* matches, int64_t cap, int64_t* match_off, uint8_t* pair_ok) {
+  return match_all(device, descriptors, img_off, n_img, dim, pairs, n_pairs, options, matches, cap, match_off, pair_ok, nullptr);
+}
+
+int tbm_debug_nn2(int device, const float* descriptors, const int64_t* img_off, int32_t n_img, int32_t dim, const int32_t* pairs,
+                  int64_t n_pairs, int symmetric, int32_t* best_j, float* best_d, float* second_d, uint8_t* exhaustive) {
+  if (!img_off || !pairs || !best_j || !best_d || !second_d || !exhaustive || n_img < 0 || n_pairs < 0) return -1;
+  for (int i = 0; i < n_img; ++i) if (img_off[i + 1] < img_off[i]) return -1;
+  int64_t nq = 0;
+  for (int64_t p = 0; p < n_pairs; ++p) {
+    const int a = pairs[2 * p], b = pairs[2 * p + 1];
+    if (a < 0 || a >= n_img || b < 0 || b >= n_img) return -1;
+    nq += (img_off[a + 1] - img_off[a]) + (symmetric ? img_off[b + 1] - img_off[b] : 0);
+  }
+  std::memset(exhaustive, 0, (size_t)nq);
+  // every forward query may keep its match: no ratio test, no early exit -- the decisions are not what this hook reports
+  tbm_options o;
+  tbm_options_init(&o);
+  o.keep_only_symmetric_matches = symmetric != 0; o.use_lowes_ratio = 0; o.min_num_feature_matches = 0;
+  std::vector<tbm_match> m((size_t)nq + 1);
+  std::vector<int64_t> off((size_t)n_pairs + 1);
+  std::vector<uint8_t> ok((size_t)n_pairs + 1);
+  const Nn2Out out{best_j, best_d, second_d, exhaustive};
+  return match_all(device, descriptors, img_off, n_img, dim, pairs, n_pairs, &o, m.data(), nq + 1, off.data(), ok.data(), &out);
 }
 
 }  // extern "C"

@@ -8,15 +8,15 @@
 //   1. k_nn_candidates (this file): ||x - y||^2 = ||x||^2 + ||y||^2 - 2 x.y with the 128-dimensional dot products as a TF32
 //      wgmma GEMM -- a 128-query block of image A (resident in shared memory) against 64-candidate tiles of image B streamed
 //      by TMA (cp.async.bulk.tensor, 128-byte swizzle, NSTAGE-deep ring) -- and a fused epilogue on the fp32 accumulator
-//      registers that keeps, per query row, the candidates whose score ||y||^2 - 2 x.y lies within the TF32 error margin of
-//      the running runner-up (branch-free, lists in shared memory).
+//      registers that keeps, per query row, the candidates whose score interval (||y||^2 - 2 x.y widened by its TF32 and float
+//      error bounds) reaches below the runner-up's (branch-free, lists in shared memory).
 //      Warp roles: warpgroup 0 = TMA producer (one thread), warpgroups 1 and 2 = consumers: each issues the m64n64k8 wgmmas
 //      of its 64 query rows and scans its accumulators.  Persistent CTAs over a list of work items.
 //   2. k_exact_top2: the KC candidates of every query are re-evaluated EXACTLY -- float, term by term in the reference's
 //      order without fused multiply-add, like the round-1 kernel k_nn2 -- and the best two (ties: lower index) are kept.
 // TF32 only ranks candidates; every distance that leaves the GPU, every ratio test and every tie-break is computed from
-// the exact values, so the match lists equal the CPU oracle's unless the true nearest / second-nearest neighbour is not
-// within the TF32 error margin of the running runner-up when it is seen (impossible by construction: see the epilogue comment).
+// the exact values, so the match lists equal the CPU oracle's: the reference's nearest and second-nearest neighbours always reach
+// the exact pass (see the epilogue comment; tests/test_xx_matcher_gpu_adversarial.py checks it at the inputs where it is tightest).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -155,28 +155,47 @@ __global__ void __launch_bounds__(THREADS, 1) k_nn_candidates(const __grid_const
     // Accumulator layout of m64n64 (per warp w of the warpgroup, lane l): d[4j + 2i + c] = row 16w + l/4 + 8i, column 8j + 2(l%4) + c.
     // A thread therefore owns two query rows (i = 0, 1) and one column quarter (l % 4) of each: 16 of the 64 columns of every tile.
     //
-    // Branch-free streaming selection.  Per (row, quarter) the thread keeps the running two smallest scores m1 <= m2 of
-    // score(n) = ||y_n||^2 - 2 x.y_n over ITS columns (three min/max per element) and appends an element to its candidate list in
-    // shared memory -- one predicated 8-byte store, no branch, no divergence -- whenever
-    //     score(n) < m2 + margin(n),
-    // where margin(n) is at least twice the worst-case TF32 error of a score.  wgmma .tf32 uses 10 mantissa bits of each operand
-    // (relative operand error < 2^-10 truncating, <= 2^-11 rounding), so |d score| <= 2 * 2^-9 sum_k |x_k y_k|:
-    //   * NONNEG (every descriptor component >= 0: SIFT, RootSIFT, any histogram descriptor): sum_k |x_k y_k| = x.y, read off the
-    //     accumulator itself: margin(n) = 2^-8 x.y_n (1 + 2^-6)  (truncation errors are one-sided there, so 1 x the bound suffices;
-    //     with rounding the bound halves and 2 x it is the same number);
-    //   * otherwise: sum_k |x_k y_k| <= ||x|| ||y|| <= (||x||^2 + ||y||^2) / 2:  margin(n) = 2^-8 (||x||^2 + ||y_n||^2).
-    // An element that is among the two nearest of the whole image in exact arithmetic is a fortiori among the two nearest of its
-    // quarter: it passes the test when it is seen (m2 only decreases) and stays below every later m2 + margin, so it survives the
-    // compactions (a list that grows past 8 drops the entries above the current limit).  At the end of an item the four quarters of
-    // a row merge their (m1, m2) by shuffles; the entries within the margin of the row's own runner-up -- the same test on the whole
-    // row -- are written to the KC slots of the query for the exact pass.  A list that fills up, or a row with more than KC such
-    // entries (a dense cluster of near-identical candidates), flags the row: the exact pass then scans every candidate of that query.
+    // Branch-free streaming selection.  Every element n of the row (query x, candidate y_n) gets an interval [lo_n, up_n] of
+    // float scores that must contain the reference's distance D_n = fl(sum_k (x_k - y_nk)^2) minus ||x||^2, and an element can only be
+    // among the two nearest when lo_n <= the second smallest up of the row: were lo_n > up_c1, up_c2 for two other elements, both
+    // would be strictly nearer than n in the reference's own arithmetic.  Per (row, quarter) the thread keeps the running two smallest
+    // up, m1 <= m2 (three min/max per element), and appends an element to its candidate list in shared memory -- one predicated
+    // 8-byte store, no branch, no divergence -- whenever lo_n <= m2 (m2 only decreases, so a true top-2 element passes when it is
+    // seen and at every later compaction).  lo and up are the computed score ||y_n||^2 - 2 acc_n minus / plus the bound of its
+    // distance from D_n - ||x||^2 (X = ||x||^2, Y = ||y_n||^2, A = sum_k |x_k y_nk|, p = x.y_n, d = X + Y - 2p):
+    //   * TF32 operands: wgmma .tf32 uses the top 10 mantissa bits of each fp32 operand and ignores the low 13 -- truncation toward
+    //     zero, which an H100 does (tests/test_xx_matcher_gpu_adversarial.py::test_tf32_operands_are_truncated pins it): an operand
+    //     loses < 2^-10 of itself.  The products are exact in fp32; the fp32 accumulation of 128 of them errs <= 2^-16 A either way.
+    //     With non-negative data every product only shrinks: acc - p lies in [-2^-9 A (1 + 2^-7), +2^-16 A], i.e. the score
+    //     ||y||^2 - 2 acc errs by at most 2^-8 A (1 + 2^-7) upward and 2^-15 A downward; with signed data by 2^-8 A either way;
+    //   * the float norm nrm[n] (k_row_norms' order) differs from Y by <= 2^-19 Y, the reference's sum D_n from d by <= 2^-17 d (a
+    //     left-to-right sum of 128 rounded squares), and the roundings of lo / up add <= 2^-22 (X + Y + A): <= 2^-16 (X + Y) with d <= X + Y;
+    //   * NONNEG (every descriptor component >= 0: SIFT, RootSIFT, any histogram descriptor): A = p = acc (1 + 2^-9), d <= X + Y:
+    //       lo = Y (1 - 2^-16) - acc (2 + 2^-8 + 2^-14) - 2^-16 X,   up = Y (1 + 2^-16) - acc (2 - 2^-14) + 2^-16 X;
+    //   * otherwise A <= ||x|| ||y|| <= (X + Y) / 2 and d <= 2 (X + Y):
+    //       lo = Y (1 - b) - 2 acc - b X,   up = Y (1 + b) - 2 acc + b X,   b = 2^-9 (1 + 2^-4).
+    // The norm terms keep the interval open where the TF32 term vanishes (a zero query or candidate, disjoint supports: x.y = 0),
+    // and since lo_n <= up_n always, the comparison "<=" keeps the runner-up itself and every exact tie.  The kernel keeps lo and up
+    // scaled (lo', up' below: one FMA each off the plain norm, as cheap as a bare score) and compares lo' with the running limit
+    // kK m2' + kX X (one more FMA per element).  m1', m2' start at 2^126 instead of +inf, so the limit stays finite: out-of-range
+    // columns of the last tile (lo' = up' = +inf) are never appended.
+    // At the end of an item the four quarters of a row merge their (m1, m2) by shuffles; the entries within the row's own limit are
+    // written to the KC slots of the query for the exact pass.  A list that fills up, or a row with more than KC such entries (a dense
+    // cluster of near-identical candidates), flags the row: the exact pass then scans every candidate of that query.
     // The first tile is scanned twice: once only to establish m1, m2 (otherwise every element of it would be appended).
     const int g = warp / 4 - 1;              // consumer warpgroup: query rows [64 g, 64 g + 64) of the block
     const int wl = warp & 3;
     const int et = threadIdx.x - 128;        // 0..255 among the consumer threads
     const int cq = lane & 3;                 // column quarter
-    const float kInf = __int_as_float(0x7f800000);
+    const float kInf = __int_as_float(0x7f800000), kBig = 0x1p126f;
+    // the interval scaled per side so that both ends are one FMA off the plain norm: lo' = (lo + b X) / (1 - b) = fmaf(kLo, acc, nrm),
+    // up' = (up - b X) / (1 + b) = fmaf(kUp, acc, nrm); lo <= up_2 + b X  <=>  lo' <= kK up'_2 + kX X  (kK = (1 + b) / (1 - b),
+    // kX = 2 b / (1 - b)).  Each constant is rounded away from the tighter side (|kLo|, kK, kX up; |kUp| down).
+    // NONNEG: b = 2^-16, lo / up TF32 coefficients 2 + 2^-8 + 2^-14 / 2 - 2^-14;  otherwise: b = 2^-9 + 2^-13, both 2
+    constexpr float kLo = NONNEG ? -0x1.0083020000000p+1f : -0x1.00884a0000000p+1f;
+    constexpr float kUp = NONNEG ? -0x1.fffa000000000p+0f : -0x1.fef0900000000p+0f;
+    constexpr float kK = NONNEG ? 0x1.0002020000000p+0f : 0x1.0110920000000p+0f;
+    constexpr float kX = NONNEG ? 0x1.0001020000000p-15f : 0x1.1090ce0000000p-8f;
     constexpr uint32_t kStride = NLISTS * (uint32_t)sizeof(uint2);   // bytes between consecutive entries of one list
     const uint32_t a_base = smem_addr(sA + g * 4 * PANEL_BYTES);
     float acc[32];
@@ -186,14 +205,14 @@ __global__ void __launch_bounds__(THREADS, 1) k_nn_candidates(const __grid_const
     for (int it = blockIdx.x; it < n_items; it += gridDim.x, ++itc) {
       const WorkItem w = items[it];
       int row[2];
-      float m1[2], m2[2], nx8[2];
+      float m1[2], m2[2], xm[2];
       uint32_t c_base[2], c_last[2], wp[2];
       int ovf[2];
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
         row[i] = g * WG_ROWS + wl * 16 + (lane >> 2) + 8 * i;   // query row of this thread inside the block
-        m1[i] = kInf; m2[i] = kInf;
-        nx8[i] = (!NONNEG && row[i] < w.a_rows) ? 0.00390625f * __ldg(nrm + w.a_row0 + row[i]) : 0.0f;  // 2^-8 ||x||^2 (general margin only)
+        m1[i] = kBig; m2[i] = kBig;
+        xm[i] = row[i] < w.a_rows ? kX * __ldg(nrm + w.a_row0 + row[i]) : 0.0f;  // the row term of the limit
         // wp = shared-memory address of the next append; it saturates at the last slot, and a list that reaches the last slot
         // counts as overflowed (capacity CAP - 4 entries between two maintenance points)
         c_base[i] = smem_addr(sC + i * 256 + et);
@@ -233,7 +252,7 @@ __global__ void __launch_bounds__(THREADS, 1) k_nn_candidates(const __grid_const
         // one predicated 8-byte store + pointer bump per element; the pointer is clamped to the last slot once per FOUR elements
         // (TBM_CLAMP): at most four appends can happen in between, and the lists keep four spare slots behind c_last for them
 #define TBM_APPEND(I, VAL, J)                                                                                           \
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.lt.f32 p, %1, %2;\n\t@p st.shared.v2.b32 [%0], {%3, %4};\n\t@p add.u32 %0, %0, %5;\n\t}"      \
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.le.f32 p, %1, %2;\n\t@p st.shared.v2.b32 [%0], {%3, %4};\n\t@p add.u32 %0, %0, %5;\n\t}"      \
                : "+r"(wp[I]) : "f"(VAL), "f"(lim), "r"(__float_as_uint(VAL)), "r"(J), "n"(kStride) : "memory")
 #define TBM_CLAMP(I) wp[I] = min(wp[I], c_last[I])
 #pragma unroll
@@ -243,18 +262,19 @@ __global__ void __launch_bounds__(THREADS, 1) k_nn_candidates(const __grid_const
             for (int j = 0; j < 8; ++j)
 #pragma unroll
               for (int c = 0; c < 2; ++c) {
-                const float sc = fmaf(-2.0f, acc[4 * j + 2 * i + c], nn[j][c]);
-                m2[i] = fminf(m2[i], fmaxf(m1[i], sc));
-                m1[i] = fminf(m1[i], sc);
+                const float up = fmaf(kUp, acc[4 * j + 2 * i + c], nn[j][c]);
+                m2[i] = fminf(m2[i], fmaxf(m1[i], up));
+                m1[i] = fminf(m1[i], up);
               }
-            const float lim = NONNEG ? m2[i] : m2[i] + nx8[i];
+          }
+          if (t == 0) {
+            const float lim = fmaf(m2[i], kK, xm[i]);
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
 #pragma unroll
               for (int c = 0; c < 2; ++c) {
-                const float dotv = acc[4 * j + 2 * i + c];
-                const float val = fmaf(NONNEG ? dotv : nn[j][c], NONNEG ? -0.00396728515625f : -0.00390625f, fmaf(-2.0f, dotv, nn[j][c]));
-                TBM_APPEND(i, val, jg + 8 * j + c);
+                const float lo = fmaf(kLo, acc[4 * j + 2 * i + c], nn[j][c]);
+                TBM_APPEND(i, lo, jg + 8 * j + c);
               }
               if (j & 1) TBM_CLAMP(i);
             }
@@ -264,12 +284,12 @@ __global__ void __launch_bounds__(THREADS, 1) k_nn_candidates(const __grid_const
 #pragma unroll
               for (int c = 0; c < 2; ++c) {
                 const float dotv = acc[4 * j + 2 * i + c];
-                const float sc = fmaf(-2.0f, dotv, nn[j][c]);
-                const float val = fmaf(NONNEG ? dotv : nn[j][c], NONNEG ? -0.00396728515625f : -0.00390625f, sc);   // score minus the candidate's margin
-                const float lim = NONNEG ? m2[i] : m2[i] + nx8[i];
-                TBM_APPEND(i, val, jg + 8 * j + c);
-                m2[i] = fminf(m2[i], fmaxf(m1[i], sc));
-                m1[i] = fminf(m1[i], sc);
+                const float lo = fmaf(kLo, dotv, nn[j][c]);
+                const float up = fmaf(kUp, dotv, nn[j][c]);
+                const float lim = fmaf(m2[i], kK, xm[i]);
+                TBM_APPEND(i, lo, jg + 8 * j + c);
+                m2[i] = fminf(m2[i], fmaxf(m1[i], up));
+                m1[i] = fminf(m1[i], up);
               }
               if (j & 1) TBM_CLAMP(i);
             }
@@ -278,12 +298,12 @@ __global__ void __launch_bounds__(THREADS, 1) k_nn_candidates(const __grid_const
           ovf[i] |= wp[i] == c_last[i];
           if (wp[i] > c_base[i] + 8 * kStride) {
             const int cnt = (int)((wp[i] - c_base[i]) / kStride);
-            const float lim = m2[i] + nx8[i];
+            const float lim = fmaf(m2[i], kK, xm[i]);
             uint2* myC = sC + i * 256 + et;
             int k = 0;
             for (int e = 0; e < cnt; ++e) {
               const uint2 ce = myC[e * NLISTS];
-              if (__uint_as_float(ce.x) < lim) { myC[k * NLISTS] = ce; ++k; }
+              if (__uint_as_float(ce.x) <= lim) { myC[k * NLISTS] = ce; ++k; }
             }
             wp[i] = c_base[i] + (uint32_t)k * kStride;
           }
@@ -301,11 +321,11 @@ __global__ void __launch_bounds__(THREADS, 1) k_nn_candidates(const __grid_const
           r2 = fminf(fmaxf(r1, o1), fminf(r2, o2));
           r1 = fminf(r1, o1);
         }
-        const float lim = r2 + nx8[i];   // the final runner-up of the row: only entries within its margin can matter
+        const float lim = fmaf(r2, kK, xm[i]);   // the row's final limit: only entries with lo' <= it can be among the two nearest
         const uint2* myC = sC + i * 256 + et;
         const int cnt = (int)((wp[i] - c_base[i]) / kStride);
         int k = 0;
-        for (int e = 0; e < cnt; ++e) k += __uint_as_float(myC[e * NLISTS].x) < lim;
+        for (int e = 0; e < cnt; ++e) k += __uint_as_float(myC[e * NLISTS].x) <= lim;
         int before = 0, total = 0, any_ovf = 0;
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
@@ -322,7 +342,7 @@ __global__ void __launch_bounds__(THREADS, 1) k_nn_candidates(const __grid_const
             int n = before;
             for (int e = 0; e < cnt; ++e) {
               const uint2 ce = myC[e * NLISTS];
-              if (__uint_as_float(ce.x) < lim) o[n++] = (int)ce.y;
+              if (__uint_as_float(ce.x) <= lim) o[n++] = (int)ce.y;
             }
             if (cq == 3) for (int q = total; q < KC; ++q) o[q] = -1;
           }

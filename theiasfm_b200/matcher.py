@@ -8,7 +8,8 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libtheia_matcher_b200.so")
 _LIB = None
-EXPORTED_SYMBOLS = ["tbm_options_init", "tbm_match_all", "tbm_debug_postprocess", "tbm_debug_last_timing", "tbm_debug_exact_top2"]
+EXPORTED_SYMBOLS = ["tbm_options_init", "tbm_match_all", "tbm_debug_postprocess", "tbm_debug_last_timing", "tbm_debug_exact_top2",
+                    "tbm_debug_nn2"]
 
 
 class tbm_match(C.Structure):
@@ -35,6 +36,8 @@ def lib():
         L.tbm_debug_last_timing.argtypes = [C.POINTER(C.c_double)]
         L.tbm_debug_last_timing.restype = None
         L.tbm_debug_exact_top2.argtypes = [C.c_int, fp, C.c_int64, ip, ip, ip, ip, C.c_int64, ip, fp, fp]
+        L.tbm_debug_nn2.argtypes = [C.c_int, fp, C.POINTER(C.c_int64), C.c_int32, C.c_int32, ip, C.c_int64, C.c_int, ip, fp, fp,
+                                    C.POINTER(C.c_uint8)]
         _LIB = L
     return _LIB
 
@@ -59,6 +62,41 @@ def exact_top2(descriptors, q_row, b_row0, b_rows, cand, device=0):
     return rc, bj, bd, sd
 
 
+def _pack(descriptor_sets, pairs):
+    dim = descriptor_sets[0].shape[1]
+    off = np.zeros(len(descriptor_sets) + 1, np.int64)
+    off[1:] = np.cumsum([len(d) for d in descriptor_sets])
+    desc = np.ascontiguousarray(np.concatenate(descriptor_sets, axis=0), np.float32) if off[-1] else np.zeros((0, dim), np.float32)
+    pr = np.ascontiguousarray(np.array(pairs, np.int32).reshape(-1, 2))
+    return dim, off, desc, pr
+
+
+def nn2(descriptor_sets, pairs, symmetric=True, device=0):
+    """tbm_debug_nn2: the per-query nearest / second-nearest results of tbm_match_all's search stage.
+    Returns (rc, [per pair: dict(fwd=(best_j, best_d, second_d, exhaustive), rev=(...) or None)])."""
+    dim, off, desc, pr = _pack(descriptor_sets, pairs)
+    sizes = np.diff(off)
+    nq = int(sum(sizes[a] + (sizes[b] if symmetric else 0) for a, b in pr))
+    bj = np.zeros(max(nq, 1), np.int32); bd = np.zeros(max(nq, 1), np.float32); sd = np.zeros(max(nq, 1), np.float32)
+    ex = np.zeros(max(nq, 1), np.uint8)
+    fp, ip = C.POINTER(C.c_float), C.POINTER(C.c_int32)
+    rc = lib().tbm_debug_nn2(device, desc.ctypes.data_as(fp), off.ctypes.data_as(C.POINTER(C.c_int64)), len(descriptor_sets), dim,
+                             pr.ctypes.data_as(ip), len(pr), int(bool(symmetric)), bj.ctypes.data_as(ip), bd.ctypes.data_as(fp),
+                             sd.ctypes.data_as(fp), ex.ctypes.data_as(C.POINTER(C.c_uint8)))
+    res, q = [], 0
+    for a, b in pr:
+        part = {}
+        for key, n in (("fwd", sizes[a]), ("rev", sizes[b] if symmetric else None)):
+            if n is None:
+                part[key] = None
+                continue
+            n = int(n)
+            part[key] = (bj[q:q + n], bd[q:q + n], sd[q:q + n], ex[q:q + n].astype(bool))
+            q += n
+        res.append(part)
+    return rc, res
+
+
 def default_options(**kw):
     o = tbm_options()
     lib().tbm_options_init(C.byref(o))
@@ -71,11 +109,7 @@ def match_all(descriptor_sets, pairs, options=None, device=0):
     """descriptor_sets: list of [n_i, dim] float32 arrays; pairs: [(i, j), ...].
     Returns (rc, [list of (f1, f2, dist) per pair], [ok per pair])."""
     options = options or default_options()
-    dim = descriptor_sets[0].shape[1]
-    off = np.zeros(len(descriptor_sets) + 1, np.int64)
-    off[1:] = np.cumsum([len(d) for d in descriptor_sets])
-    desc = np.ascontiguousarray(np.concatenate(descriptor_sets, axis=0), np.float32) if off[-1] else np.zeros((0, dim), np.float32)
-    pr = np.ascontiguousarray(np.array(pairs, np.int32).reshape(-1, 2))
+    dim, off, desc, pr = _pack(descriptor_sets, pairs)
     cap = int(sum(len(descriptor_sets[i]) for i, _ in pairs)) + 1
     out = (tbm_match * cap)()
     moff = np.zeros(len(pr) + 1, np.int64)
