@@ -1,4 +1,4 @@
-// host_segments.cc -- CPU check of the "fast" segmented warp reduction (TBA_FAST_SEG=1): tba_segments.h's run_last_lane is the
+// host_segments.cc -- CPU check of the "fast" segmented warp reduction (seg_reduce_to): tba_segments.h's run_last_lane is the
 // product's code; the two reductions are emulated lane by lane with the shuffle semantics of __shfl_down_sync (a lane whose
 // source is out of range keeps its own value).
 #include <cstdint>

@@ -85,6 +85,9 @@ SCENES = {
                          intrinsics_to_optimize=_abi.INTR_NONE),
     "pinhole_focal_pp": dict(n_cam=9, n_pt=200, obs_per_pt=4, model=_abi.MODEL_PINHOLE, shared_intrinsics=False, seed=25,
                              intrinsics_to_optimize=_abi.INTR_FOCAL_LENGTH | _abi.INTR_PRINCIPAL_POINTS),
+    # tracks cut to 3..48 observations: 'long' tiles (tracks > 32 observations, per-point sums combined across warps in shared
+    # memory) after the normal ones, with exactly-32 / 33-observation tracks at the boundary
+    "long_short": dict(n_cam=120, n_pt=260, obs_per_pt=48, seed=41, track_lengths=(3, 7, 31, 32, 33, 48)),
 }
 
 
@@ -95,8 +98,26 @@ def _width(loss, default):
     return 80.0 if loss == _abi.LOSS_TUKEY else default
 
 
+def _cut_tracks(p, lengths):
+    """Every track keeps its first n observations, n drawn from `lengths` per point."""
+    rng = np.random.default_rng(1)
+    keep = np.ones(p.n_obs, bool)
+    target = {q: int(rng.choice(lengths)) for q in range(p.n_pt)}
+    seen = np.zeros(p.n_pt, int)
+    for i in range(p.n_obs):
+        q = int(p.obs_pt[i])
+        seen[q] += 1
+        keep[i] = seen[q] <= target[q]
+    return _abi.Problem(p.ext, p.ext_const, p.cam_group, p.group_model, p.intr, p.group_const_mask, p.pt, p.pt_const,
+                        p.obs_cam[keep], p.obs_pt[keep], p.obs_xy[keep])
+
+
 def _scene(name, constants=False):
-    p = synthetic.make_scene(**SCENES[name])
+    kw = dict(SCENES[name])
+    lengths = kw.pop("track_lengths", None)
+    p = synthetic.make_scene(**kw)
+    if lengths is not None:
+        p = _cut_tracks(p, lengths)
     if constants:
         p.ext_const[1] = _abi.EXT_ALL_CONST
         p.ext_const[2] = _abi.EXT_POSITION_CONST
@@ -258,17 +279,7 @@ def test_edge_cases(eng, oracle):
 def test_long_tracks_use_the_cta_level_path(eng, oracle):
     """Tracks with more than 32 observations live in 'long' tiles (per-point sums combined across warps in shared
     memory); mixed with short tracks and exactly-32 / 33-observation tracks at the boundary."""
-    p = synthetic.make_scene(n_cam=120, n_pt=260, obs_per_pt=48, seed=41)
-    rng = np.random.default_rng(1)
-    keep = np.ones(p.n_obs, bool)
-    target = {q: int(rng.choice([3, 7, 31, 32, 33, 48])) for q in range(p.n_pt)}
-    seen = np.zeros(p.n_pt, int)
-    for i in range(p.n_obs):
-        q = int(p.obs_pt[i])
-        seen[q] += 1
-        keep[i] = seen[q] <= target[q]
-    p = _abi.Problem(p.ext, p.ext_const, p.cam_group, p.group_model, p.intr, p.group_const_mask, p.pt, p.pt_const,
-                     p.obs_cam[keep], p.obs_pt[keep], p.obs_xy[keep])
+    p = _scene("long_short")
     counts = np.bincount(p.obs_pt, minlength=p.n_pt)
     assert (counts > 32).sum() > 20 and (counts == 32).sum() > 5 and (counts < 32).sum() > 20
     po, pg = p.copy(), p.copy()

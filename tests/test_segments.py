@@ -1,4 +1,4 @@
-"""The experiment switch TBA_FAST_SEG=1 replaces the key shuffles of the segmented warp reduction by a run structure derived from
+"""The streaming kernels replace the key shuffles of the segmented warp reduction by a run structure derived from
 the ballot of the run heads (theiasfm_b200/csrc/tba_segments.h).  Checked on the CPU: run_last_lane against brute force for random
 run layouts (including the tile layouts the pack produces: points, then unique negative keys for padding lanes), and the two
 reductions -- emulated with __shfl_down_sync's semantics -- give bit-identical results in every lane that starts a run."""

@@ -147,11 +147,7 @@ struct tba_context {
   DevBuf<uint8_t> d_inner_status;
   int64_t inner_passes = 0;
   bool has_ext_models = false;  // some group uses FISHEYE / FOV / DIVISION_UNDISTORTION: EXT kernel instantiations
-  bool exp_tred = true;     // transposed RED emission (warp_red_rows) in k_linearize / k_precond_ext / rhs / matvec; TBA_TRED=0: the round-1 lane-per-row REDs
-  bool exp_lin_occ = true;  // k_linearize compiled for 3 CTAs/SM (80 registers, ~130 bytes of spills); TBA_LIN_OCC=2: 2 CTAs/SM, 128 registers
   double trace_pcg_gpu_ms = 0.0;  // TBA_TRACE_LM: device-side span of the PCG launches (first launch .. state copy), summed over a minimize
-  bool pcg_fused = true;    // one vector kernel per CG iteration (k_pcg_fused, grid barriers between its phases); TBA_PCG=split: k_pcg_c / k_pcg_a / k_pcg_b
-  bool stream_schur = true; // persistent streaming k_schur_stream over the normal tiles; TBA_MATVEC=tile: the tile-per-CTA k_schur everywhere
   int n_normal_tiles = 0;   // tiles whose tracks fit a warp slice (they precede the long tiles)
   // fused matvec + all-reduce over peer memory (P2pDev, tba_kernels.cuh): world > 1, every peer reachable, TBA_P2P != 0
   bool p2p_enabled = true, p2p_ok = false, p2p_use = false;
@@ -293,20 +289,8 @@ int stage_linearize(tba_context* c, double* cost, double* fixed, bool* ok, doubl
     if (c->has_ext_models) {  // FISHEYE / FOV / DIVISION_UNDISTORTION present: the dual-number instantiation, all 10 columns
       auto kfn = k_linearize<0x3FFu, true>;
       LAUNCH(c, kfn, P.n_tiles, TILE, 0, P, lin_g(c), lin_cn(c), c->rep.p);
-    } else if (c->exp_lin_occ && c->exp_tred) {
-#define F(M) { auto kfn = k_linearize<M, false, true, 3>; LAUNCH(c, kfn, P.n_tiles, TILE, 0, P, lin_g(c), lin_cn(c), c->rep.p); }
-      DISPATCH_IMASK(c->imask, F)
-#undef F
-    } else if (c->exp_lin_occ) {
-#define F(M) { auto kfn = k_linearize<M, false, false, 3>; LAUNCH(c, kfn, P.n_tiles, TILE, 0, P, lin_g(c), lin_cn(c), c->rep.p); }
-      DISPATCH_IMASK(c->imask, F)
-#undef F
-    } else if (c->exp_tred) {
-#define F(M) { auto kfn = k_linearize<M, false, true>; LAUNCH(c, kfn, P.n_tiles, TILE, 0, P, lin_g(c), lin_cn(c), c->rep.p); }
-      DISPATCH_IMASK(c->imask, F)
-#undef F
     } else {
-#define F(M) LAUNCH(c, k_linearize<M>, P.n_tiles, TILE, 0, P, lin_g(c), lin_cn(c), c->rep.p)
+#define F(M) { auto kfn = k_linearize<M, false>; LAUNCH(c, kfn, P.n_tiles, TILE, 0, P, lin_g(c), lin_cn(c), c->rep.p); }
       DISPATCH_IMASK(c->imask, F)
 #undef F
     }
@@ -443,7 +427,7 @@ template <int MODE>
 int launch_schur(tba_context* c, const double* xs, double* y, const int* done, const P2pDev& pp = P2pDev()) {
   DevProblem& P = c->P;
   int first_tile = 0;
-  if (c->stream_schur && c->exp_tred && c->n_normal_tiles > 0) {
+  if (c->n_normal_tiles > 0) {
     const int n_slices = c->n_normal_tiles * (TILE / 32);
 #define F(M) { using Cfg = StreamCfg<M, MODE>; auto kfn = k_schur_stream<M, MODE>; \
                const int grid = std::max(1, std::min(c->n_sm, (n_slices + Cfg::NW - 1) / Cfg::NW)); \
@@ -454,15 +438,9 @@ int launch_schur(tba_context* c, const double* xs, double* y, const int* done, c
   }
   const int rest = P.n_tiles - first_tile;
   if (rest > 0) {
-    if (c->exp_tred || MODE == 2) {
-#define F(M) { auto kfn = k_schur<M, MODE, true>; LAUNCH(c, kfn, rest, TILE, schur_smem(c), P, xs, y, c->rep.p, done, first_tile); }
-      DISPATCH_IMASK(c->imask, F)
+#define F(M) { auto kfn = k_schur<M, MODE>; LAUNCH(c, kfn, rest, TILE, schur_smem(c), P, xs, y, c->rep.p, done, first_tile); }
+    DISPATCH_IMASK(c->imask, F)
 #undef F
-    } else {
-#define F(M) { auto kfn = k_schur<M, MODE, false>; LAUNCH(c, kfn, rest, TILE, schur_smem(c), P, xs, y, c->rep.p, done, first_tile); }
-      DISPATCH_IMASK(c->imask, F)
-#undef F
-    }
   }
   return TBA_OK;
 }
@@ -486,9 +464,9 @@ int stage_prepare(tba_context* c, double radius, bool* ok, bool defer_flag = fal
   else CUDA_OK(c, cudaMemsetAsync(c->y.p, 0, (size_t)P.ncs * sizeof(double), c->stream));
   if (P.n_tiles > 0) {
     // normal tiles: ONE streaming pass over J for the reduced rhs and both families of SCHUR_JACOBI blocks (k_prepare_stream);
-    // long tiles (and TBA_MATVEC=tile / IDENTITY preconditioner): the three tile kernels
+    // long tiles: the three tile kernels (IDENTITY preconditioner: launch_schur splits the rhs pass the same way)
     int first_tile = 0;
-    if (c->stream_schur && c->exp_tred && precond && c->n_normal_tiles > 0) {
+    if (precond && c->n_normal_tiles > 0) {
       const int n_slices = c->n_normal_tiles * (TILE / 32);
       const int pb = prof_begin(c);
 #define F(M) { using Cfg = PrepCfg<M>; auto kfn = k_prepare_stream<M>; \
@@ -502,15 +480,9 @@ int stage_prepare(tba_context* c, double radius, bool* ok, bool defer_flag = fal
     const int rest = P.n_tiles - first_tile;
     if (rest > 0 && precond) {
       const int pb_ext = prof_begin(c);
-      if (c->exp_tred) {
-#define F(M) { auto kfn = k_precond_ext<M, true>; LAUNCH(c, kfn, rest, TILE, 0, P, c->Sblk.p, first_tile); }
-        DISPATCH_IMASK(c->imask, F)
-#undef F
-      } else {
 #define F(M) LAUNCH(c, k_precond_ext<M>, rest, TILE, 0, P, c->Sblk.p, first_tile)
-        DISPATCH_IMASK(c->imask, F)
+      DISPATCH_IMASK(c->imask, F)
 #undef F
-      }
       prof_end(c, 2, pb_ext);
       if (c->NI > 0) {
         const size_t smem = (size_t)TILE * 4 * c->NI * sizeof(double) + 2 * TILE * sizeof(int);
@@ -525,7 +497,7 @@ int stage_prepare(tba_context* c, double radius, bool* ok, bool defer_flag = fal
       const int pb_rhs = prof_begin(c);
       if (first_tile == 0) { const int rc1 = launch_schur<1>(c, nullptr, yr, nullptr); if (rc1) return rc1; }
       else {
-#define F(M) { auto kfn = k_schur<M, 1, true>; LAUNCH(c, kfn, rest, TILE, schur_smem(c), P, nullptr, yr, c->rep.p, nullptr, first_tile); }
+#define F(M) { auto kfn = k_schur<M, 1>; LAUNCH(c, kfn, rest, TILE, schur_smem(c), P, nullptr, yr, c->rep.p, nullptr, first_tile); }
         DISPATCH_IMASK(c->imask, F)
 #undef F
       }
@@ -557,7 +529,7 @@ int stage_prepare(tba_context* c, double radius, bool* ok, bool defer_flag = fal
 
 const int* st_done(const PcgState* st) { return reinterpret_cast<const int*>(reinterpret_cast<const char*>(st) + offsetof(PcgState, done)); }
 
-// The fused path is available when the whole problem runs through the streaming kernel (no long tiles, the default kernels).
+// The fused path is available when the whole problem runs through the streaming kernel (no long tiles).
 bool p2p_matvec_possible(const tba_context* c) { return c->p2p_ok && c->p2p_use; }
 
 // defer_fold: the caller folds the shared-intrinsics replica rows itself (k_pcg_a / k_pcg_reset_bz; one GPU only).
@@ -606,10 +578,14 @@ int stage_pcg(tba_context* c, int* iters, int* status, bool* system_ok = nullptr
   double* fold_rep = fold_in_a ? c->rep.p : nullptr;
   const bool p2p = p2p_matvec_possible(c);  // multi-GPU: the matvec pushes its partial sums to the peers, k_pcg_a sums the inbox
   int* zero_ctr = p2p ? c->p2p_ctr : nullptr;
-  // c->pcg_fused (default): ONE vector kernel per CG iteration -- phases A and B of iteration k and phase C of iteration k + 1 in
-  // k_pcg_fused, grid barriers in between -- i.e. two launches per iteration with the matvec; TBA_PCG=split (and the SIMT emulation
-  // build, which cannot run a grid barrier): the three kernels
-  const bool fused = c->pcg_fused;
+  // On the GPU: ONE vector kernel per CG iteration -- phases A and B of iteration k and phase C of iteration k + 1 in k_pcg_fused,
+  // grid barriers in between -- i.e. two launches per iteration with the matvec.  The SIMT emulation build runs the CTAs of a
+  // launch one after the other and so cannot run a grid barrier: it launches the three kernels (the same device functions).
+#ifdef TBA_EMULATE
+  constexpr bool fused = false;
+#else
+  constexpr bool fused = true;
+#endif
   PcgVectors V;
   V.sm = c->sm.p; V.D2 = c->D2.p; V.b = c->b.p; V.Minv_c = c->Minv_c.p; V.Minv_i = c->Minv_i.p;
   V.p = c->p.p; V.q = c->z.p; V.x = c->x.p; V.r = c->r.p; V.z = c->z2.p; V.xs = c->xs.p; V.y = c->y.p;
@@ -951,15 +927,7 @@ int tba_create(int device, int rank, int world_size, const void* nccl_unique_id,
   tba_context* c = new tba_context();
   c->device = device; c->rank = rank; c->world = world_size;
   tba_options_init(&c->opt);
-  { const char* e = getenv("TBA_MATVEC"); c->stream_schur = !(e != nullptr && e[0] == 't'); }
-  { const char* e = getenv("TBA_PCG"); c->pcg_fused = !(e != nullptr && e[0] == 's'); }
-#ifdef TBA_EMULATE
-  c->pcg_fused = false;  // the emulator runs the CTAs of a launch one after the other: no grid barrier (the three phases are the same device functions)
-#endif
   { const char* e = getenv("TBA_P2P"); c->p2p_enabled = !(e != nullptr && e[0] == '0'); }
-  // the transposed RED emission and the 3-CTA/SM linearise are the defaults; TBA_TRED=0 / TBA_LIN_OCC=2 select the round-1 kernels
-  { const char* e = getenv("TBA_LIN_OCC"); c->exp_lin_occ = !(e != nullptr && e[0] == '2'); }
-  { const char* e = getenv("TBA_TRED"); c->exp_tred = !(e != nullptr && e[0] == '0'); }
   if (cudaSetDevice(device) != cudaSuccess || cudaDeviceGetAttribute(&c->n_sm, cudaDevAttrMultiProcessorCount, device) != cudaSuccess || cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking) != cudaSuccess ||
       cudaMallocHost(&c->h_scal, 64 * sizeof(double)) != cudaSuccess || cudaMallocHost(&c->h_st, sizeof(PcgState)) != cudaSuccess) {
     delete c;
@@ -1225,7 +1193,7 @@ int tba_upload(tba_context* c, const tba_options* options, const tba_problem* p)
   P.slot_cam = c->slot_cam.p; P.slot_pt = c->slot_pt.p; P.slot_flags = c->slot_flags.p; P.slot_run = c->slot_run.p;
   P.tile_pt_begin = c->tile_pt_begin.p; P.tile_nruns = c->tile_nruns.p; P.tile_flags = c->tile_flags.p; P.xy = c->xy.p; P.J = c->J.p; P.res = c->res.p;
   P.Hpp = c->Hpp.p; P.gp = c->gp.p; P.Mp = c->Mp.p; P.sp = c->sp.p; P.dpt = c->dpt.p; P.pt_const = c->pt_const.p;
-  { const char* e = getenv("TBA_ABLATE"); P.ablate = e ? atoi(e) : 0; }  // timing diagnostics only (wrong results): see k_schur
+  { const char* e = getenv("TBA_ABLATE"); P.ablate = e ? atoi(e) : 0; }  // timing diagnostics only (wrong results): see k_schur_stream
   if (c->NI > 0) {
     const int smem = TILE * 4 * c->NI * (int)sizeof(double) + 2 * TILE * (int)sizeof(int);
 #define F(M) CUDA_OK(c, cudaFuncSetAttribute(k_precond_intr<M>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem))
@@ -1235,11 +1203,9 @@ int tba_upload(tba_context* c, const tba_options* options, const tba_problem* p)
   {
     const int smem = (int)schur_smem(c);
 #define F(M)                                                                                                        \
-  CUDA_OK(c, cudaFuncSetAttribute(k_schur<M, 0, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));        \
-  CUDA_OK(c, cudaFuncSetAttribute(k_schur<M, 0, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));       \
-  CUDA_OK(c, cudaFuncSetAttribute(k_schur<M, 1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));        \
-  CUDA_OK(c, cudaFuncSetAttribute(k_schur<M, 1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));       \
-  CUDA_OK(c, cudaFuncSetAttribute(k_schur<M, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));        \
+  CUDA_OK(c, cudaFuncSetAttribute(k_schur<M, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));              \
+  CUDA_OK(c, cudaFuncSetAttribute(k_schur<M, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));              \
+  CUDA_OK(c, cudaFuncSetAttribute(k_schur<M, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));              \
   CUDA_OK(c, cudaFuncSetAttribute(k_schur_stream<M, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)StreamCfg<M, 0>::SMEM)); \
   CUDA_OK(c, cudaFuncSetAttribute(k_schur_stream<M, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)StreamCfg<M, 1>::SMEM)); \
   CUDA_OK(c, cudaFuncSetAttribute(k_schur_stream<M, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)StreamCfg<M, 2>::SMEM)); \
@@ -1256,7 +1222,7 @@ int tba_upload(tba_context* c, const tba_options* options, const tba_problem* p)
     if (rcp) return rcp;
     c->p2p_use = false;
     if (c->world > 1 && c->p2p_ok) {
-      const double mine = (c->stream_schur && c->exp_tred && c->n_normal_tiles > 0 && c->n_normal_tiles == n_tiles) ? 0.0 : 1.0;
+      const double mine = (c->n_normal_tiles == n_tiles && c->n_normal_tiles > 0) ? 0.0 : 1.0;
       double others = 0.0;
       CUDA_OK(c, cudaMemcpyAsync(c->scal2.p, &mine, 8, cudaMemcpyHostToDevice, c->stream));
       const int r2 = allreduce_sum(c, c->scal2.p, 1);

@@ -29,8 +29,8 @@ struct DevProblem {
   int ncs;                     // n_cam*6 + n_group*10 (camera-space vector length)
   int single_group;            // n_group == 1: block-reduce the intrinsics accumulations
   int loss_type; double loss_width;
-  int ablate;                  // TBA_ABLATE (timing diagnostics of the matvec, results are WRONG when non-zero): bit0 no camera-side
-                               // REDs, bit1 no x gather, bit2 no shared-intrinsics warp sums, bit3 no segmented reduction
+  int ablate;                  // TBA_ABLATE (timing diagnostics of the streaming matvec, results are WRONG when non-zero): bit0 no
+                               // camera-side REDs, bit1 no x gather, bit3 no segmented reduction
   // parameters: current x and candidate
   double *ext, *intr, *pt, *ext_c, *intr_c, *pt_c;
   const int* cam_group; const int* group_model;
@@ -94,7 +94,7 @@ __device__ __forceinline__ double seg_reduce(double v, int key, int lane) {
 
 // The same reduction when the run structure is known from a ballot of the run heads: lane + o belongs to lane's run iff
 // lane + o <= run_last (runs are contiguous), so the key does not have to be shuffled along with every value -- 5 shuffles per
-// reduced value instead of 10 (experiment switch TBA_FAST_SEG=1; bit-identical sums: same additions in the same order).
+// reduced value instead of 10 (bit-identical sums: same additions in the same order).
 __device__ __forceinline__ double seg_reduce_to(double v, int run_last, int lane) {
 #pragma unroll
   for (int o = 1; o < 32; o <<= 1) {
@@ -115,7 +115,7 @@ __device__ __forceinline__ void red_add(double* p, double v) {
 #endif
 }
 
-// Experiment TBA_TRED=1 ("transposed" RED emission).  A lane-per-observation RED of an N-double camera row touches 32
+// "Transposed" RED emission.  A lane-per-observation RED of an N-double camera row touches 32
 // different 32-byte sectors per instruction (32 cameras), i.e. N x 32 sector operations at the L2 atomic units, which
 // is what bounds these kernels (one L2 sector operation per lane and RED).  Here
 // the warp first stages its 32 rows in shared memory ([32][N] doubles, lane-major) and then emits them element-major:
@@ -189,9 +189,13 @@ __device__ __forceinline__ size_t wslice(int tile, int warp, int rows) { return 
 // gradient / squared column norms (fp64 RED to global) and cost / failure counters (replicas).
 // Normal tiles: a point never straddles a warp -> per-point sums by warp-shuffle segmented reduction only, no
 // block barrier.  Long tiles (tracks > 32 observations): combined across warps in shared memory.
-template <uint32_t IMASK, bool EXT = false, bool TRED = false, int MINB = 1>
-__global__ void __launch_bounds__(TILE, MINB) k_linearize(DevProblem P, double* __restrict__ g_cs, double* __restrict__ cn_cs,
-                                                    double* __restrict__ rep) {
+// Built for 3 CTAs/SM, with the camera-side rows of normal tiles staged and emitted element-major (warp_red_rows).  The EXT
+// instantiation (dual numbers for FISHEYE / FOV / DIVISION_UNDISTORTION) needs the registers: 1 CTA/SM, and one RED per lane
+// and row element on every tile.
+template <uint32_t IMASK, bool EXT = false>
+__global__ void __launch_bounds__(TILE, EXT ? 1 : 3) k_linearize(DevProblem P, double* __restrict__ g_cs, double* __restrict__ cn_cs,
+                                                           double* __restrict__ rep) {
+  constexpr bool STAGED_RED = !EXT;
   constexpr int NI = popcount10(IMASK);
   constexpr int NJ = 14 + 2 * NI;
   __shared__ double s_acc[MAXP][14];
@@ -283,8 +287,8 @@ __global__ void __launch_bounds__(TILE, MINB) k_linearize(DevProblem P, double* 
     }
   }
   // camera-side gradient and squared column norms: J_c = [-h Ja | Jw]
-  if (TRED && !long_tile) {
-    // experimental (TBA_TRED=1): both 6-rows staged per warp in the (idle on normal tiles) s_acc area, emitted element-major
+  if (STAGED_RED && !long_tile) {
+    // both 6-rows staged per warp in the (idle on normal tiles) s_acc area, emitted element-major
     double gv[6], cv[6];
 #pragma unroll
     for (int j = 0; j < 3; ++j) {
@@ -294,7 +298,7 @@ __global__ void __launch_bounds__(TILE, MINB) k_linearize(DevProblem P, double* 
       gv[3 + j] = Jw[j] * r[0] + Jw[3 + j] * r[1];
       cv[3 + j] = Jw[j] * Jw[j] + Jw[3 + j] * Jw[3 + j];
     }
-    static_assert(MAXP * 14 >= (TILE / 32) * (2 * 32 * 6 + 16), "s_acc too small for the TRED staging");
+    static_assert(MAXP * 14 >= (TILE / 32) * (2 * 32 * 6 + 16), "s_acc too small for the row staging");
     double* stage = &s_acc[0][0] + warp * (2 * 32 * 6 + 16);
     int* sbase = reinterpret_cast<int*>(stage + 2 * 32 * 6);
     warp_stage_row<6>(stage, sbase, gv, valid ? cam * 6 : -1, lane);
@@ -600,15 +604,13 @@ __device__ __forceinline__ void sym4_mul(const double* __restrict__ M, const dou
 // ---------------------------------------------------- TMA (bulk async copy) helpers
 #ifdef TBA_EMULATE
 // CPU emulation build (tests/emu/cuda_emu.h): the bulk copy is a memcpy by the issuing lane, the mbarrier a flag the other lanes
-// poll (yielding to the fiber scheduler), the bulk reduction an in-place add.
+// poll (yielding to the fiber scheduler).
 // *bar counts the completed phases: the issuing lane's sequence "expect_tx, bulk copy, bulk copy ..." runs without a yield in
 // between, so a phase is complete as soon as its expect_tx is visible; wait(parity) passes once phase `parity` is over.
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t) { *bar = 0; }
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t) { *bar += 1; }
 __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t*) { memcpy(dst, src, bytes); }
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) { while ((*bar & 1u) == parity) emu_yield(); }
-__device__ __forceinline__ void bulk_red_add_f64(double* dst, const double* src_smem, uint32_t bytes) { for (uint32_t i = 0; i < bytes / 8; ++i) dst[i] += src_smem[i]; }
-__device__ __forceinline__ void bulk_commit_and_wait_read() {}
 __device__ __forceinline__ void fence_proxy_async_smem() {}
 #else
 // cp.async.bulk global -> shared::cta completing on an mbarrier (SASS: UBLKCP + SYNCS.ARRIVE.TRANS64).
@@ -639,18 +641,6 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
 // Never a silent hang: a bulk copy that does not land within ~2 s (4e9 SM cycles) is a bug -- report it and abort the kernel
 // (the launch then fails with a CUDA error that the engine returns to the caller).
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-#ifdef TBA_MBAR_SIMPLE
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "WAIT_%=:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-      "@p bra DONE_%=;\n\t"
-      "bra WAIT_%=;\n\t"
-      "DONE_%=:\n\t}" ::"r"(smem_u32(bar)),
-      "r"(parity)
-      : "memory");
-  return;
-#endif
   if (mbar_try_wait(bar, parity)) return;
   const long long t0 = clock64();
   while (!mbar_try_wait(bar, parity)) {
@@ -659,18 +649,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
       __trap();
     }
   }
-}
-
-// Bulk reduction shared -> global (TMA): dst[0..bytes) += src[0..bytes) element-wise in fp64, asynchronously.
-// bytes multiple of 16, both addresses 16-byte aligned.  Experimental path (TBA_MATVEC_BULKRED=1): replaces the six
-// per-observation RED.ADD.F64 of the matvec by ONE 48-byte bulk reduction issued from a staged shared-memory row.
-__device__ __forceinline__ void bulk_red_add_f64(double* dst, const double* src_smem, uint32_t bytes) {
-  asm volatile("cp.reduce.async.bulk.global.shared::cta.bulk_group.add.f64 [%0], [%1], %2;" ::"l"(dst), "r"(smem_u32(src_smem)), "r"(bytes)
-               : "memory");
-}
-__device__ __forceinline__ void bulk_commit_and_wait_read() {
-  asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-  asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
 }
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
@@ -683,15 +661,15 @@ __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.p
 // All with the UNSCALED stored Jacobian; the Jacobi scaling lives in xs (= s .* x), M and the
 // post-scaling of y (k_pcg_* kernels).  xs: camera-space vector [n_cam*6 | n_group*10].
 //
-// Every WARP is autonomous on a normal tile: lane 0 issues one TMA bulk copy of the warp's contiguous slice of the
-// compact Jacobian (NJ x 32 doubles) [+ residuals] into the warp's shared-memory stage, completing on the warp's
-// own mbarrier; meanwhile all lanes gather their camera's x block (3 x 128-bit loads) and the head lanes fetch
-// M_p, so the gather latency overlaps the copy.  Per-point sums: warp-shuffle segmented reduction (a point's
-// observations are contiguous lanes of ONE warp), u_p = M_p t_p on the head lane, broadcast back by shuffle.
-// Camera-side sums: fp64 RED.ADD to global; shared-intrinsics sums: warp reduce + RED to a replica row.
-// No block barrier on this path.  Long tiles (tracks > 32 observations) combine the per-point sums across warps in
-// shared memory (two block barriers).  Dynamic shared memory: TILE * (NJ + 2) doubles.
-template <uint32_t IMASK, int MODE, bool TRED = true>
+// k_schur runs over the LONG tiles (tracks of 33..256 observations), one CTA per tile; k_schur_stream takes the normal
+// tiles, which the pack puts before every long tile.  Lane 0 of every warp issues one TMA bulk copy of the warp's contiguous
+// slice of the compact Jacobian (NJ x 32 doubles) [+ residuals] into the warp's shared-memory stage, completing on the
+// warp's own mbarrier; meanwhile all lanes gather their camera's x block (3 x 128-bit loads), so the gather latency overlaps
+// the copy.  Per-point sums: warp-shuffle segmented reduction, combined across warps in shared memory (a point's observations
+// may straddle warps; two block barriers), u_p = M_p t_p by one thread per point.  Camera-side sums: staged per warp and
+// emitted element-major (warp_red_rows); intrinsics sums: warp reduce + RED to a replica row (one shared group) or one RED
+// per lane.  Correct for any tile.  Dynamic shared memory: TILE * (NJ + 2) doubles.
+template <uint32_t IMASK, int MODE>
 __global__ void __launch_bounds__(TILE, (14 + 2 * popcount10(IMASK)) <= 20 ? 4 : 2) k_schur(DevProblem P, const double* __restrict__ xs, double* __restrict__ y,
                                                 double* __restrict__ rep, const int* __restrict__ done_flag, int tile0) {
   constexpr int NI = popcount10(IMASK);
@@ -715,11 +693,8 @@ __global__ void __launch_bounds__(TILE, (14 + 2 * popcount10(IMASK)) <= 20 ? 4 :
     bulk_g2s(sJ, P.J + wslice(tile, warp, NJ), jbytes, &s_bar[warp]);
     if (MODE != 0) bulk_g2s(sR, P.res + wslice(tile, warp, 2), rbytes, &s_bar[warp]);
   }
-  const bool long_tile = (P.tile_flags[tile] & 1) != 0;
   const int p0 = P.tile_pt_begin[tile], npt = P.tile_pt_begin[tile + 1] - p0;
-  if (long_tile) {
-    for (int i = tid; i < npt * 4; i += TILE) (&s_t[0][0])[i] = 0.0;
-  }
+  for (int i = tid; i < npt * 4; i += TILE) (&s_t[0][0])[i] = 0.0;
   const size_t slot = (size_t)tile * TILE + tid;
   const int cam = P.slot_cam[slot];
   const bool valid = cam >= 0;
@@ -729,10 +704,10 @@ __global__ void __launch_bounds__(TILE, (14 + 2 * popcount10(IMASK)) <= 20 ? 4 :
   double xi[NI + 1];
   if (valid) {
     pl = P.slot_pt[slot] - p0;
-    grp = (TRED && P.single_group) ? 0 : P.cam_group[cam];  // TRED: no 32-sector gather when one group owns everything
+    grp = P.single_group ? 0 : P.cam_group[cam];  // no 32-sector gather when one group owns everything
     h = P.pt[(size_t)(p0 + pl) * 4 + 3];
     if (MODE != 1) {
-      const double2* x2 = reinterpret_cast<const double2*>(xs + (size_t)((MODE == 0 && (P.ablate & 2)) ? lane : cam) * 6);
+      const double2* x2 = reinterpret_cast<const double2*>(xs + (size_t)cam * 6);
       xa = __ldg(x2); xb = __ldg(x2 + 1); xc = __ldg(x2 + 2);
       if (NI > 0) {
         const double* xg = xs + P.ne + (size_t)grp * 10;
@@ -743,15 +718,7 @@ __global__ void __launch_bounds__(TILE, (14 + 2 * popcount10(IMASK)) <= 20 ? 4 :
   }
   const int prev = __shfl_up_sync(0xffffffffu, pl, 1);
   const bool head = lane == 0 || prev != pl;
-  const unsigned heads = __ballot_sync(0xffffffffu, head);
-  // head lanes prefetch M_p (normal tiles)
-  double2 m01 = make_double2(0.0, 0.0), m23 = m01, m45 = m01, m67 = m01, m89 = m01;
-  if (!long_tile && head && valid) {
-    const double2* M2 = reinterpret_cast<const double2*>(P.Mp + (size_t)(p0 + pl) * 10);
-    m01 = __ldg(M2); m23 = __ldg(M2 + 1); m45 = __ldg(M2 + 2); m67 = __ldg(M2 + 3); m89 = __ldg(M2 + 4);
-  }
-  if (long_tile) __syncthreads();  // s_t zeroed
-  __syncwarp();
+  __syncthreads();  // s_t zeroed
   mbar_wait(&s_bar[warp], 0);  // this warp's slice landed in shared memory
   const double* Jt = sJ + lane;
 #define JA(j) Jt[(j) * 32]
@@ -776,45 +743,26 @@ __global__ void __launch_bounds__(TILE, (14 + 2 * popcount10(IMASK)) <= 20 ? 4 :
     t[0] = JA(0) * w0 + JA(3) * w1; t[1] = JA(1) * w0 + JA(4) * w1; t[2] = JA(2) * w0 + JA(5) * w1;
     t[3] = JH(0) * w0 + JH(1) * w1;
   }
-  if (MODE == 0 && (P.ablate & 8)) {
-  } else {
 #pragma unroll
-    for (int j = 0; j < 4; ++j) t[j] = seg_reduce(t[j], pl, lane);
-  }
-  double u0, u1, u2, u3;
-  if (!long_tile) {
-    u0 = m01.x * t[0] + m01.y * t[1] + m23.x * t[2] + m23.y * t[3];
-    u1 = m01.y * t[0] + m45.x * t[1] + m45.y * t[2] + m67.x * t[3];
-    u2 = m23.x * t[0] + m45.y * t[1] + m67.y * t[2] + m89.x * t[3];
-    u3 = m23.y * t[0] + m67.x * t[1] + m89.x * t[2] + m89.y * t[3];
-    if (MODE == 2 && head && valid) {
-      double2* d = reinterpret_cast<double2*>(P.dpt + (size_t)(p0 + pl) * 4);
-      d[0] = make_double2(-u0, -u1);
-      d[1] = make_double2(-u2, -u3);
-    }
-    const int hl = run_head_lane(heads, lane);
-    u0 = __shfl_sync(0xffffffffu, u0, hl); u1 = __shfl_sync(0xffffffffu, u1, hl);
-    u2 = __shfl_sync(0xffffffffu, u2, hl); u3 = __shfl_sync(0xffffffffu, u3, hl);
-  } else {
-    if (head && valid) {
+  for (int j = 0; j < 4; ++j) t[j] = seg_reduce(t[j], pl, lane);
+  if (head && valid) {
 #pragma unroll
-      for (int j = 0; j < 4; ++j) atomicAdd(&s_t[pl][j], t[j]);
-    }
-    __syncthreads();
-    if (tid < npt) {
-      const double tt[4] = {s_t[tid][0], s_t[tid][1], s_t[tid][2], s_t[tid][3]};
-      double uu[4];
-      sym4_mul(P.Mp + (size_t)(p0 + tid) * 10, tt, uu);
-      s_t[tid][0] = uu[0]; s_t[tid][1] = uu[1]; s_t[tid][2] = uu[2]; s_t[tid][3] = uu[3];
-      if (MODE == 2) {
-        double* d = P.dpt + (size_t)(p0 + tid) * 4;
-        d[0] = -uu[0]; d[1] = -uu[1]; d[2] = -uu[2]; d[3] = -uu[3];
-      }
-    }
-    __syncthreads();
-    u0 = u1 = u2 = u3 = 0.0;
-    if (valid) { u0 = s_t[pl][0]; u1 = s_t[pl][1]; u2 = s_t[pl][2]; u3 = s_t[pl][3]; }
+    for (int j = 0; j < 4; ++j) atomicAdd(&s_t[pl][j], t[j]);
   }
+  __syncthreads();
+  if (tid < npt) {
+    const double tt[4] = {s_t[tid][0], s_t[tid][1], s_t[tid][2], s_t[tid][3]};
+    double uu[4];
+    sym4_mul(P.Mp + (size_t)(p0 + tid) * 10, tt, uu);
+    s_t[tid][0] = uu[0]; s_t[tid][1] = uu[1]; s_t[tid][2] = uu[2]; s_t[tid][3] = uu[3];
+    if (MODE == 2) {
+      double* d = P.dpt + (size_t)(p0 + tid) * 4;
+      d[0] = -uu[0]; d[1] = -uu[1]; d[2] = -uu[2]; d[3] = -uu[3];
+    }
+  }
+  __syncthreads();
+  double u0 = 0.0, u1 = 0.0, u2 = 0.0, u3 = 0.0;
+  if (valid) { u0 = s_t[pl][0]; u1 = s_t[pl][1]; u2 = s_t[pl][2]; u3 = s_t[pl][3]; }
   double z0 = 0.0, z1 = 0.0;
   if (valid) {
     z0 = w0 - (JA(0) * u0 + JA(1) * u1 + JA(2) * u2 + JH(0) * u3);
@@ -830,10 +778,8 @@ __global__ void __launch_bounds__(TILE, (14 + 2 * popcount10(IMASK)) <= 20 ? 4 :
     }
     mcc = warp_sum(mcc);
     if (lane == 0) red_add(rr + 23, mcc);
-    return;
-  }
-  if (TRED) {
-    // camera-side contributions staged per warp and emitted element-major (warp_red_rows); TBA_TRED=0: one RED per lane and row element
+  } else {
+    // camera-side contributions staged per warp and emitted element-major (warp_red_rows)
     double yv[6];
 #pragma unroll
     for (int j = 0; j < 3; ++j) yv[j] = valid ? -h * (JA(j) * z0 + JA(3 + j) * z1) : 0.0;
@@ -846,45 +792,18 @@ __global__ void __launch_bounds__(TILE, (14 + 2 * popcount10(IMASK)) <= 20 ? 4 :
     int* sbase = reinterpret_cast<int*>(sJ + 32 * 6);
     warp_stage_row<6>(sJ, sbase, yv, valid ? cam * 6 : -1, lane);
     __syncwarp();
-    if (!(MODE == 0 && (P.ablate & 1))) warp_red_rows<6>(y, sJ, sbase, lane);
+    warp_red_rows<6>(y, sJ, sbase, lane);
     if (NI > 0) {
       if (P.single_group) {
-        if (MODE == 0 && (P.ablate & 4)) {
-          double v = 0.0;
-#pragma unroll
-          for (int j = 0; j < NI; ++j) v += yi[j];
-          if (v == 1.2345e300) red_add(rr, v);
-        } else {
 #pragma unroll
         for (int j = 0; j < NI; ++j) {
           const double v = warp_sum(yi[j]);
           if (lane == 0) red_add(rr + nth_bit(IMASK, j), v);
         }
-        }
       } else if (valid) {
 #pragma unroll
         for (int j = 0; j < NI; ++j) red_add(y + P.ne + (size_t)grp * 10 + nth_bit(IMASK, j), yi[j]);
       }
-    }
-    return;
-  }
-  if (valid) {
-    double* yc = y + (size_t)cam * 6;
-#pragma unroll
-    for (int j = 0; j < 3; ++j) red_add(yc + j, -h * (JA(j) * z0 + JA(3 + j) * z1));
-#pragma unroll
-    for (int j = 0; j < 3; ++j) red_add(yc + 3 + j, JW(j) * z0 + JW(3 + j) * z1);
-  }
-  if (NI > 0) {
-    if (P.single_group) {
-#pragma unroll
-      for (int j = 0; j < NI; ++j) {
-        const double v = warp_sum(valid ? JI(j) * z0 + JI(NI + j) * z1 : 0.0);
-        if (lane == 0) red_add(rr + nth_bit(IMASK, j), v);
-      }
-    } else if (valid) {
-#pragma unroll
-      for (int j = 0; j < NI; ++j) red_add(y + P.ne + (size_t)grp * 10 + nth_bit(IMASK, j), JI(j) * z0 + JI(NI + j) * z1);
     }
   }
 #undef JA
@@ -1106,23 +1025,10 @@ k_schur_stream(DevProblem P, const double* __restrict__ xs, double* __restrict__
 #define JI(j) Jt[(14 + (j)) * 32]
     double w0 = 0.0, w1 = 0.0, r0 = 0.0, r1 = 0.0;
     // the whole row set of this lane in registers: every element of J is read from shared memory exactly once
-    double ja[6], jh[2], jw[6], ji[2 * NI + 1];
+    double ja[6], jh[2];
 #pragma unroll
     for (int j = 0; j < 6; ++j) ja[j] = JA(j);
     jh[0] = JH(0); jh[1] = JH(1);
-#ifndef TBA_STREAM_CACHE_J
-#define TBA_STREAM_CACHE_J 0
-#endif
-    if (TBA_STREAM_CACHE_J && MODE != 2) {
-#pragma unroll
-      for (int j = 0; j < 6; ++j) jw[j] = JW(j);
-#pragma unroll
-      for (int j = 0; j < 2 * NI; ++j) ji[j] = JI(j);
-    }
-#undef JW
-#undef JI
-#define JW(j) ((TBA_STREAM_CACHE_J && MODE != 2) ? jw[j] : Jt[(6 + (j)) * 32])
-#define JI(j) ((TBA_STREAM_CACHE_J && MODE != 2) ? ji[j] : Jt[(14 + (j)) * 32])
     if (valid) {
       if (MODE != 0) { r0 = sR[lane]; r1 = sR[32 + lane]; }
       if (MODE != 1) {
@@ -1530,85 +1436,52 @@ k_prepare_stream(DevProblem P, double* __restrict__ y, double* __restrict__ Sc, 
 // ------------------------------------------- SCHUR_JACOBI preconditioner blocks
 // Extrinsics blocks: S_cc = sum_o J_c^T Q_o J_c with Q_o = I_2 - J_p M_p J_p^T (a view observes a track once).
 // Sc: [n_cam][21] upper triangle, unscaled (scaling + D^2 + inversion in k_precond_finish).
-template <uint32_t IMASK, bool TRED = false>
+// The 21 block entries of every observation are staged per warp and emitted element-major (warp_red_rows).
+template <uint32_t IMASK>
 __global__ void __launch_bounds__(TILE) k_precond_ext(DevProblem P, double* __restrict__ Sc, int tile0) {
   constexpr int NI = popcount10(IMASK);
   constexpr int NJ = 14 + 2 * NI;
   const int tile = tile0 + blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const size_t slot = (size_t)tile * TILE + tid;
   const int cam = P.slot_cam[slot];
-  if (TRED) {
-    // experimental (TBA_TRED=1): the 21 block entries of every observation staged per warp, emitted element-major
-    __shared__ double s_stage[TILE / 32][32 * 21];
-    __shared__ int s_base[TILE / 32][32];
-    double v[21];
+  __shared__ double s_stage[TILE / 32][32 * 21];
+  __shared__ int s_base[TILE / 32][32];
+  double v[21];
 #pragma unroll
-    for (int j = 0; j < 21; ++j) v[j] = 0.0;
-    if (cam >= 0) {
-      const double* Jt = P.J + wslice(tile, warp, NJ) + lane;
-      double Ja[6], Jw[6], Jh[2];
+  for (int j = 0; j < 21; ++j) v[j] = 0.0;
+  if (cam >= 0) {
+    const double* Jt = P.J + wslice(tile, warp, NJ) + lane;
+    double Ja[6], Jw[6], Jh[2];
 #pragma unroll
-      for (int j = 0; j < 6; ++j) Ja[j] = Jt[j * 32];
+    for (int j = 0; j < 6; ++j) Ja[j] = Jt[j * 32];
 #pragma unroll
-      for (int j = 0; j < 6; ++j) Jw[j] = Jt[(6 + j) * 32];
-      Jh[0] = Jt[12 * 32];
-      Jh[1] = Jt[13 * 32];
-      const int pt = P.slot_pt[slot];
-      const double h = P.pt[(size_t)pt * 4 + 3];
-      const double* M = P.Mp + (size_t)pt * 10;
-      const double jp0[4] = {Ja[0], Ja[1], Ja[2], Jh[0]}, jp1[4] = {Ja[3], Ja[4], Ja[5], Jh[1]};
-      double m0[4], m1[4];
-      sym4_mul(M, jp0, m0);
-      sym4_mul(M, jp1, m1);
-      const double q00 = 1.0 - (jp0[0] * m0[0] + jp0[1] * m0[1] + jp0[2] * m0[2] + jp0[3] * m0[3]);
-      const double q01 = -(jp0[0] * m1[0] + jp0[1] * m1[1] + jp0[2] * m1[2] + jp0[3] * m1[3]);
-      const double q11 = 1.0 - (jp1[0] * m1[0] + jp1[1] * m1[1] + jp1[2] * m1[2] + jp1[3] * m1[3]);
-      double c0[6], c1[6];
+    for (int j = 0; j < 6; ++j) Jw[j] = Jt[(6 + j) * 32];
+    Jh[0] = Jt[12 * 32];
+    Jh[1] = Jt[13 * 32];
+    const int pt = P.slot_pt[slot];
+    const double h = P.pt[(size_t)pt * 4 + 3];
+    const double* M = P.Mp + (size_t)pt * 10;
+    const double jp0[4] = {Ja[0], Ja[1], Ja[2], Jh[0]}, jp1[4] = {Ja[3], Ja[4], Ja[5], Jh[1]};
+    double m0[4], m1[4];
+    sym4_mul(M, jp0, m0);
+    sym4_mul(M, jp1, m1);
+    const double q00 = 1.0 - (jp0[0] * m0[0] + jp0[1] * m0[1] + jp0[2] * m0[2] + jp0[3] * m0[3]);
+    const double q01 = -(jp0[0] * m1[0] + jp0[1] * m1[1] + jp0[2] * m1[2] + jp0[3] * m1[3]);
+    const double q11 = 1.0 - (jp1[0] * m1[0] + jp1[1] * m1[1] + jp1[2] * m1[2] + jp1[3] * m1[3]);
+    double c0[6], c1[6];
 #pragma unroll
-      for (int j = 0; j < 3; ++j) { c0[j] = -h * Ja[j]; c1[j] = -h * Ja[3 + j]; c0[3 + j] = Jw[j]; c1[3 + j] = Jw[3 + j]; }
-      int n = 0;
+    for (int j = 0; j < 3; ++j) { c0[j] = -h * Ja[j]; c1[j] = -h * Ja[3 + j]; c0[3 + j] = Jw[j]; c1[3 + j] = Jw[3 + j]; }
+    int n = 0;
 #pragma unroll
-      for (int a = 0; a < 6; ++a) {
-        const double qa0 = q00 * c0[a] + q01 * c1[a], qa1 = q01 * c0[a] + q11 * c1[a];
+    for (int a = 0; a < 6; ++a) {
+      const double qa0 = q00 * c0[a] + q01 * c1[a], qa1 = q01 * c0[a] + q11 * c1[a];
 #pragma unroll
-        for (int b = a; b < 6; ++b) { v[n] = qa0 * c0[b] + qa1 * c1[b]; ++n; }
-      }
+      for (int b = a; b < 6; ++b) { v[n] = qa0 * c0[b] + qa1 * c1[b]; ++n; }
     }
-    warp_stage_row<21>(s_stage[warp], s_base[warp], v, cam >= 0 ? cam * 21 : -1, lane);
-    __syncwarp();
-    warp_red_rows<21>(Sc, s_stage[warp], s_base[warp], lane);
-    return;
   }
-  if (cam < 0) return;
-  const double* Jt = P.J + wslice(tile, warp, NJ) + lane;
-  double Ja[6], Jw[6], Jh[2];
-#pragma unroll
-  for (int j = 0; j < 6; ++j) Ja[j] = Jt[j * 32];
-#pragma unroll
-  for (int j = 0; j < 6; ++j) Jw[j] = Jt[(6 + j) * 32];
-  Jh[0] = Jt[12 * 32];
-  Jh[1] = Jt[13 * 32];
-  const int pt = P.slot_pt[slot];
-  const double h = P.pt[(size_t)pt * 4 + 3];
-  const double* M = P.Mp + (size_t)pt * 10;
-  const double jp0[4] = {Ja[0], Ja[1], Ja[2], Jh[0]}, jp1[4] = {Ja[3], Ja[4], Ja[5], Jh[1]};
-  double m0[4], m1[4];
-  sym4_mul(M, jp0, m0);
-  sym4_mul(M, jp1, m1);
-  const double q00 = 1.0 - (jp0[0] * m0[0] + jp0[1] * m0[1] + jp0[2] * m0[2] + jp0[3] * m0[3]);
-  const double q01 = -(jp0[0] * m1[0] + jp0[1] * m1[1] + jp0[2] * m1[2] + jp0[3] * m1[3]);
-  const double q11 = 1.0 - (jp1[0] * m1[0] + jp1[1] * m1[1] + jp1[2] * m1[2] + jp1[3] * m1[3]);
-  double c0[6], c1[6];
-#pragma unroll
-  for (int j = 0; j < 3; ++j) { c0[j] = -h * Ja[j]; c1[j] = -h * Ja[3 + j]; c0[3 + j] = Jw[j]; c1[3 + j] = Jw[3 + j]; }
-  double* S = Sc + (size_t)cam * 21;
-  int n = 0;
-#pragma unroll
-  for (int a = 0; a < 6; ++a) {
-    const double qa0 = q00 * c0[a] + q01 * c1[a], qa1 = q01 * c0[a] + q11 * c1[a];
-#pragma unroll
-    for (int b = a; b < 6; ++b) { red_add(S + n, qa0 * c0[b] + qa1 * c1[b]); ++n; }
-  }
+  warp_stage_row<21>(s_stage[warp], s_base[warp], v, cam >= 0 ? cam * 21 : -1, lane);
+  __syncwarp();
+  warp_red_rows<21>(Sc, s_stage[warp], s_base[warp], lane);
 }
 
 // Intrinsics blocks: S_gg = sum_o J_i^T J_i - sum_(p,g) W^T M_p W, W = sum_{o in p and g} J_p^T J_i.

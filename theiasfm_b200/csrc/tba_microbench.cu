@@ -42,7 +42,7 @@ __global__ void k_gather(const double* __restrict__ x, unsigned n_rows, int reps
 }
 
 // Design questions, measured by every bench run before the timed solve (tba_microbench_ex):
-// k_red_rows: the element-major ("transposed", TBA_TRED) emission -- lanes 6q..6q+5 of a warp add to the 6 consecutive doubles
+// k_red_rows: the element-major ("transposed", warp_red_rows) emission -- lanes 6q..6q+5 of a warp add to the 6 consecutive doubles
 // of one random 48-byte row (2 sectors), i.e. 32 elements cover ~11 sectors instead of 32.  G elements/s, comparable to k_red.
 __global__ void k_red_rows(double* y, unsigned n_rows, int reps) {
   const unsigned gid = blockIdx.x * blockDim.x + threadIdx.x;
