@@ -339,6 +339,12 @@ int tba_debug_pack(const tba_problem* problem, int64_t cap_slots, int64_t* sizes
                    int16_t* slot_run, uint8_t* slot_flags, double* xy, int64_t* slot_orig, int32_t* pk2caller,
                    int32_t* tile_pt_begin, int32_t* tile_nruns, uint8_t* tile_flags, double* mask);
 int tba_debug_linearize(tba_context* ctx, double* cost);
+/* One linearisation at the current parameters, returning the raw device buffers: J [n_slots/32][NJ][32], res [n_slots/32][2][32],
+ * Hpp [n_pt][10], gp [n_pt][4] (packed points), lin [2 ncs + 3] = gradient | squared column norms | cost, fixed cost, failed
+ * evaluations.  tile_kernel != 0: the tile-per-CTA kernel over every tile instead of the streaming kernel over the normal tiles.
+ * sizes_out = {n_slots, NJ, n_pt, ncs}; with any output pointer NULL only the sizes are returned. */
+int tba_debug_linearize_raw(tba_context* ctx, int tile_kernel, int64_t* sizes_out, double* J, double* res, double* Hpp,
+                            double* gp, double* lin);
 int tba_debug_prepare_linear_system(tba_context* ctx, double radius);
 int tba_debug_schur_matvec(tba_context* ctx, const double* x_cam /*[n_cam*6]*/,
                            const double* x_intr /*[n_group*10]*/,

@@ -279,7 +279,8 @@ int read_scal(tba_context* c, const double* dev, int n, double* out) {
 // Evaluate cost / residuals / compact Jacobian / gradient / column norms at x (and Jacobi scale at iteration 0).
 // gmax != nullptr: also the gradient max norm (max |g| over the non-constant parameters), in the same all-reduce and the same
 // device->host read as the cost -- one collective and one host synchronisation per linearisation instead of two each.
-int stage_linearize(tba_context* c, double* cost, double* fixed, bool* ok, double* gmax = nullptr) {
+// tile_kernel: k_linearize over every tile, the normal ones included (the reference of k_linearize_stream in the tests).
+int stage_linearize(tba_context* c, double* cost, double* fixed, bool* ok, double* gmax = nullptr, bool tile_kernel = false) {
   DevProblem& P = c->P;
   const size_t n_lin = 2 * (size_t)P.ncs + 16 + (size_t)c->world;  // [gradient | column norms | 16 scalars | one slot per rank]
   CUDA_OK(c, cudaMemsetAsync(c->lin.p, 0, n_lin * sizeof(double), c->stream));
@@ -288,9 +289,21 @@ int stage_linearize(tba_context* c, double* cost, double* fixed, bool* ok, doubl
     const int pb = prof_begin(c);
     if (c->has_ext_models) {  // FISHEYE / FOV / DIVISION_UNDISTORTION present: the dual-number instantiation, all 10 columns
       auto kfn = k_linearize<0x3FFu, true>;
-      LAUNCH(c, kfn, P.n_tiles, TILE, 0, P, lin_g(c), lin_cn(c), c->rep.p);
+      LAUNCH(c, kfn, P.n_tiles, TILE, 0, P, lin_g(c), lin_cn(c), c->rep.p, 0);
     } else {
-#define F(M) { auto kfn = k_linearize<M, false>; LAUNCH(c, kfn, P.n_tiles, TILE, 0, P, lin_g(c), lin_cn(c), c->rep.p); }
+      // normal tiles: the persistent streaming kernel; long tiles (tracks of 33..256 observations): one CTA per tile
+      int first_tile = 0;
+      if (c->n_normal_tiles > 0 && !tile_kernel) {
+        const int n_slices = c->n_normal_tiles * (TILE / 32);
+#define F(M) { using Cfg = LinCfg<M>; auto kfn = k_linearize_stream<M>; \
+               const int grid = std::max(1, std::min(c->n_sm, (n_slices + Cfg::NW - 1) / Cfg::NW)); \
+               LAUNCH(c, kfn, grid, Cfg::NW * 32, Cfg::SMEM, P, lin_g(c), lin_cn(c), c->rep.p, n_slices); }
+        DISPATCH_IMASK(c->imask, F)
+#undef F
+        first_tile = c->n_normal_tiles;
+      }
+      const int rest = P.n_tiles - first_tile;
+#define F(M) { auto kfn = k_linearize<M, false>; LAUNCH(c, kfn, rest, TILE, 0, P, lin_g(c), lin_cn(c), c->rep.p, first_tile); }
       DISPATCH_IMASK(c->imask, F)
 #undef F
     }
@@ -1209,7 +1222,8 @@ int tba_upload(tba_context* c, const tba_options* options, const tba_problem* p)
   CUDA_OK(c, cudaFuncSetAttribute(k_schur_stream<M, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)StreamCfg<M, 0>::SMEM)); \
   CUDA_OK(c, cudaFuncSetAttribute(k_schur_stream<M, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)StreamCfg<M, 1>::SMEM)); \
   CUDA_OK(c, cudaFuncSetAttribute(k_schur_stream<M, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)StreamCfg<M, 2>::SMEM)); \
-  CUDA_OK(c, cudaFuncSetAttribute(k_prepare_stream<M>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PrepCfg<M>::SMEM));
+  CUDA_OK(c, cudaFuncSetAttribute(k_prepare_stream<M>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PrepCfg<M>::SMEM)); \
+  CUDA_OK(c, cudaFuncSetAttribute(k_linearize_stream<M>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LinCfg<M>::SMEM));
     DISPATCH_IMASK(c->imask, F)
 #undef F
   }
@@ -1932,6 +1946,25 @@ int tba_debug_linearize(tba_context* c, double* cost) {
   c->x_cost = x; c->fixed_cost = f;
   if (cost) *cost = x + f;
   return ok ? TBA_OK : TBA_ERR_INVALID_ARGUMENT;
+}
+
+int tba_debug_linearize_raw(tba_context* c, int tile_kernel, int64_t* sizes_out, double* J, double* res, double* Hpp, double* gp, double* lin) {
+  if (!c || !c->uploaded || !sizes_out) return TBA_ERR_INVALID_ARGUMENT;
+  CUDA_OK(c, cudaSetDevice(c->device));
+  const DevProblem& P = c->P;
+  sizes_out[0] = c->n_slots; sizes_out[1] = c->NJ; sizes_out[2] = P.n_pt; sizes_out[3] = P.ncs;
+  if (!J || !res || !Hpp || !gp || !lin) return TBA_OK;
+  bool ok;
+  double x, f;
+  const int rc = stage_linearize(c, &x, &f, &ok, nullptr, tile_kernel != 0);
+  if (rc) return rc;
+  CUDA_OK(c, cudaMemcpyAsync(J, P.J, (size_t)c->n_slots * c->NJ * 8, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_OK(c, cudaMemcpyAsync(res, P.res, (size_t)c->n_slots * 2 * 8, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_OK(c, cudaMemcpyAsync(Hpp, P.Hpp, (size_t)P.n_pt * 10 * 8, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_OK(c, cudaMemcpyAsync(gp, P.gp, (size_t)P.n_pt * 4 * 8, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_OK(c, cudaMemcpyAsync(lin, c->lin.p, (2 * (size_t)P.ncs + 3) * 8, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_OK(c, cudaStreamSynchronize(c->stream));
+  return TBA_OK;
 }
 
 int tba_debug_prepare_linear_system(tba_context* c, double radius) {

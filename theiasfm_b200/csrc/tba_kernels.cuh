@@ -189,17 +189,19 @@ __device__ __forceinline__ size_t wslice(int tile, int warp, int rows) { return 
 // gradient / squared column norms (fp64 RED to global) and cost / failure counters (replicas).
 // Normal tiles: a point never straddles a warp -> per-point sums by warp-shuffle segmented reduction only, no
 // block barrier.  Long tiles (tracks > 32 observations): combined across warps in shared memory.
-// Built for 3 CTAs/SM, with the camera-side rows of normal tiles staged and emitted element-major (warp_red_rows).  The EXT
-// instantiation (dual numbers for FISHEYE / FOV / DIVISION_UNDISTORTION) needs the registers: 1 CTA/SM, and one RED per lane
-// and row element on every tile.
+// One CTA per tile from tile0 on.  In a solve the non-EXT instantiation runs over the long tiles only (k_linearize_stream takes
+// the normal ones; tba_debug_linearize_raw can run it over every tile as the reference of the streaming kernel).  It is built
+// for 3 CTAs/SM, with the camera-side rows of normal tiles staged and emitted element-major (warp_red_rows).
+// The EXT instantiation (dual numbers for FISHEYE / FOV / DIVISION_UNDISTORTION) runs over every tile and needs the registers:
+// 1 CTA/SM, and one RED per lane and row element on every tile.
 template <uint32_t IMASK, bool EXT = false>
 __global__ void __launch_bounds__(TILE, EXT ? 1 : 3) k_linearize(DevProblem P, double* __restrict__ g_cs, double* __restrict__ cn_cs,
-                                                           double* __restrict__ rep) {
+                                                           double* __restrict__ rep, int tile0) {
   constexpr bool STAGED_RED = !EXT;
   constexpr int NI = popcount10(IMASK);
   constexpr int NJ = 14 + 2 * NI;
   __shared__ double s_acc[MAXP][14];
-  const int tile = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int tile = tile0 + blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const bool long_tile = (P.tile_flags[tile] & 1) != 0;
   const int p0 = P.tile_pt_begin[tile], npt = P.tile_pt_begin[tile + 1] - p0;
   if (long_tile) {
@@ -1429,6 +1431,235 @@ k_prepare_stream(DevProblem P, double* __restrict__ y, double* __restrict__ Sc, 
           ++n;
         }
       red_add(Si + idx, vsum);
+    }
+  }
+}
+
+// --------------------------------------------- K1s: persistent streaming linearisation of the normal tiles
+// k_linearize over the normal tiles, with the structure of k_schur_stream: persistent CTAs (one per SM), every warp owns a
+// contiguous range of warp slices and a private ring of NS TMA stages; one stage = the slice's measurements xy [2][32], its
+// camera / point index rows and its constness flags.  The camera parameters and the point of slice i+1 are gathered before
+// the arithmetic of slice i and consumed one iteration later.
+//   * per observation the same linearize_obs_any as k_linearize (with the camera record rounded as there, see below) and the
+//     per-point sums in the same order: J, res, Hpp and gp are bit-identical to k_linearize's; J and res keep their
+//     [slice][NJ][32] / [slice][2][32] layout (every lane stores its element of each 256-byte row);
+//   * per-point sums by ballot-driven segmented shuffle reduction (a point never straddles a warp slice of a normal tile),
+//     written by the run's head lane;
+//   * camera gradient and squared column norms staged per warp and emitted element-major (warp_red_rows);
+//   * with one shared group the intrinsics gradient / column norms, and in every case the cost / fixed cost / failure counters,
+//     stay in registers for the whole range and leave the warp once.
+template <uint32_t IMASK>
+struct LinCfg {
+  static constexpr int NI = popcount10(IMASK);
+  static constexpr int NJ = 14 + 2 * NI;
+  static constexpr int STG = 64 + 16 + 16 + 4;  // doubles per stage: xy [2][32] | cam ids (32 int) | point ids (32 int) | flags (32 bytes)
+  static constexpr int RSTG = 2 * 32 * 6 + 16;  // camera-row staging per warp: gradient [32][6] | column norms [32][6] | 32 ints
+  static constexpr int NS = 4;                  // ring depth
+  // warps per CTA, from the register budget: the body takes 191 (NI = 0) to 252 (NI = 10) registers without spilling (ptxas -v).
+  // 8 warps (two per SM sub-partition) leave 255 per thread; 10 or 12 warps leave 168, and every instantiation with NI <= 4 spills
+  static constexpr int NW = 8;
+  static constexpr size_t SMEM = (size_t)NW * (NS * STG + RSTG) * 8 + (size_t)NW * NS * 8;
+};
+
+template <uint32_t IMASK>
+__global__ void __launch_bounds__(LinCfg<IMASK>::NW * 32, 1)
+k_linearize_stream(DevProblem P, double* __restrict__ g_cs, double* __restrict__ cn_cs, double* __restrict__ rep, int n_slices) {
+  using Cfg = LinCfg<IMASK>;
+  constexpr int NI = Cfg::NI, NJ = Cfg::NJ, STG = Cfg::STG, RSTG = Cfg::RSTG, NS = Cfg::NS, NW = Cfg::NW;
+#ifdef TBA_EMULATE
+  double* s_dyn = emu::dyn_smem<double>();
+#else
+  extern __shared__ __align__(128) double s_dyn[];
+#endif
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int gw = blockIdx.x * NW + warp, GW = gridDim.x * NW;
+  const int s_begin = (int)((long long)n_slices * gw / GW), s_end = (int)((long long)n_slices * (gw + 1) / GW);
+  double* ring = s_dyn + (size_t)warp * NS * STG;
+  double* rows = s_dyn + (size_t)NW * NS * STG + (size_t)warp * RSTG;
+  int* rbase = reinterpret_cast<int*>(rows + 2 * 32 * 6);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s_dyn + (size_t)NW * (NS * STG + RSTG)) + warp * NS;
+  auto issue = [&](int stage, int slice) {  // lane 0 only
+    double* st = ring + (size_t)stage * STG;
+    mbar_expect_tx(&bars[stage], 512 + 128 + 128 + 32);
+    bulk_g2s(st, P.xy + (size_t)slice * 64, 512, &bars[stage]);
+    int* idx = reinterpret_cast<int*>(st + 64);
+    bulk_g2s(idx, P.slot_cam + (size_t)slice * 32, 128, &bars[stage]);
+    bulk_g2s(idx + 32, P.slot_pt + (size_t)slice * 32, 128, &bars[stage]);
+    bulk_g2s(st + 96, P.slot_flags + (size_t)slice * 32, 32, &bars[stage]);
+  };
+  if (lane == 0 && s_begin < s_end) {
+#pragma unroll
+    for (int k = 0; k < NS; ++k) mbar_init(&bars[k], 1);
+#pragma unroll
+    for (int k = 0; k < NS; ++k) if (s_begin + k < s_end) issue(k, s_begin + k);
+  }
+  __syncwarp();
+  double gi_acc[NI + 1], ci_acc[NI + 1];  // shared-intrinsics gradient / column norms of this lane over the whole range
+#pragma unroll
+  for (int j = 0; j < NI; ++j) { gi_acc[j] = 0.0; ci_acc[j] = 0.0; }
+  double cost_acc = 0.0, fixed_acc = 0.0, failed_acc = 0.0;
+  // ---- registers of the slice being prefetched ("n" = next): camera ext[6] + s4[4], point, group
+  int cam_n = -1, pt_n = 0, grp_n = 0;
+  unsigned heads_n = 0xffffffffu;
+  double2 e0_n = make_double2(0.0, 0.0), e1_n = e0_n, e3_n = e0_n, q0_n = e0_n, q1_n = e0_n, X01_n = e0_n, X23_n = e0_n;
+  auto prefetch = [&](int it) {
+    const int stage = it % NS;
+    mbar_wait(&bars[stage], (uint32_t)((it / NS) & 1));
+    const int* idx = reinterpret_cast<const int*>(ring + (size_t)stage * STG + 64);
+    cam_n = idx[lane];
+    pt_n = idx[32 + lane];
+    const bool valid = cam_n >= 0;
+    const int key = valid ? pt_n : -1 - lane;  // padding lanes: unique negative keys (each its own run)
+    const int prev = __shfl_up_sync(0xffffffffu, key, 1);
+    heads_n = __ballot_sync(0xffffffffu, lane == 0 || prev != key);
+    if (valid) {
+      const double2* e2 = reinterpret_cast<const double2*>(P.ext + (size_t)cam_n * 6);
+      e0_n = __ldg(e2); e1_n = __ldg(e2 + 1); e3_n = __ldg(e2 + 2);
+      const double2* q2 = reinterpret_cast<const double2*>(P.cam_s4 + (size_t)cam_n * 4);
+      q0_n = __ldg(q2); q1_n = __ldg(q2 + 1);
+      const double2* X2 = reinterpret_cast<const double2*>(P.pt + (size_t)pt_n * 4);
+      X01_n = __ldg(X2); X23_n = __ldg(X2 + 1);
+      grp_n = P.single_group ? 0 : __ldg(P.cam_group + cam_n);
+    }
+  };
+  if (s_begin < s_end) prefetch(0);
+  for (int s = s_begin, it = 0; s < s_end; ++s, ++it) {
+    // ---- take over the prefetched registers, start the prefetch of the next slice
+    const int cam = cam_n, pt = pt_n, grp = grp_n;
+    const unsigned heads = heads_n;
+    const double2 e0 = e0_n, e1 = e1_n, e3 = e3_n, q0 = q0_n, q1 = q1_n, X01 = X01_n, X23 = X23_n;
+    const bool valid = cam >= 0;
+    if (s + 1 < s_end) prefetch(it + 1);
+    // ---- slice s: its stage landed (waited for by its prefetch)
+    const int stage = it % NS;
+    const double* st = ring + (size_t)stage * STG;
+    double Ja[6] = {0, 0, 0, 0, 0, 0}, Jw[6] = {0, 0, 0, 0, 0, 0}, Jh[2] = {0, 0}, r[2] = {0, 0};
+    double Ji[2 * NI + 1];
+#pragma unroll
+    for (int j = 0; j < 2 * NI; ++j) Ji[j] = 0.0;
+    if (valid) {
+      const double Cw[6] = {e0.x, e0.y, e1.x, e1.y, e3.x, e3.y};
+      double rec[kCamRec];
+      cam_rec_expand(e1.y, e3.x, e3.y, q0.x, q0.y, q1.x, q1.y, rec);
+#ifndef TBA_EMULATE
+      // J_l[0][2] = C02 + B w1 and J_l[2][0] = C02 - B w1 rounded as nvcc compiles them in k_linearize<IMASK, false> (C02 = Cc w0 w2
+      // rounded on its own, B w1 inside the FMA).  Left to the compiler this kernel fuses the product of C02 instead, which moves
+      // J_w by one ulp for some cameras and the solver's trajectory with it.  (The emulation build contracts nothing anywhere.)
+      {
+        const double w0 = e1.y, w1 = e3.x, w2 = e3.y, B = q1.x, Cc = q1.y;
+        const double C02 = __dmul_rn(__dmul_rn(Cc, w0), w2);
+        rec[9 + 2] = fma(B, w1, C02);
+        rec[9 + 6] = fma(-B, w1, C02);
+      }
+#endif
+      double rho0 = 0.0;
+      const bool ok = linearize_obs_any<IMASK, false>(P.group_model[grp], Cw, rec, P.intr + (size_t)grp * 10, X01.x, X01.y, X23.x,
+                                                      X23.y, st[lane], st[32 + lane], P.loss_type, P.loss_width, r, rho0, Ja, Jw, Jh, Ji);
+      const bool is_fixed = (reinterpret_cast<const uint8_t*>(st + 96)[lane] & 1) != 0;
+      if (!ok) failed_acc += 1.0;
+      else if (is_fixed) fixed_acc += 0.5 * rho0;  // every block constant: Ceres removes the residual (fixed_cost)
+      else cost_acc += 0.5 * rho0;
+      if (!ok || is_fixed) {
+#pragma unroll
+        for (int j = 0; j < 6; ++j) { Ja[j] = 0.0; Jw[j] = 0.0; }
+        Jh[0] = Jh[1] = 0.0; r[0] = r[1] = 0.0;
+#pragma unroll
+        for (int j = 0; j < 2 * NI; ++j) Ji[j] = 0.0;
+      }
+    }
+    {
+      double* Jt = P.J + (size_t)s * NJ * 32 + lane;
+#pragma unroll
+      for (int j = 0; j < 6; ++j) Jt[j * 32] = Ja[j];
+#pragma unroll
+      for (int j = 0; j < 6; ++j) Jt[(6 + j) * 32] = Jw[j];
+      Jt[12 * 32] = Jh[0];
+      Jt[13 * 32] = Jh[1];
+#pragma unroll
+      for (int j = 0; j < 2 * NI; ++j) Jt[(14 + j) * 32] = Ji[j];
+      double* rt = P.res + (size_t)s * 64 + lane;
+      rt[0] = r[0];
+      rt[32] = r[1];
+    }
+    // per-point blocks: H_pp = J_p^T J_p (10, row-major upper), g_p = J_p^T r with J_p = [Ja | Jh]
+    {
+      const double jp0[4] = {Ja[0], Ja[1], Ja[2], Jh[0]}, jp1[4] = {Ja[3], Ja[4], Ja[5], Jh[1]};
+      double acc[14];
+      int n = 0;
+#pragma unroll
+      for (int a = 0; a < 4; ++a)
+#pragma unroll
+        for (int b = a; b < 4; ++b) acc[n++] = jp0[a] * jp0[b] + jp1[a] * jp1[b];
+#pragma unroll
+      for (int a = 0; a < 4; ++a) acc[10 + a] = jp0[a] * r[0] + jp1[a] * r[1];
+      const int last = run_last_lane_dev(heads, lane);
+#pragma unroll
+      for (int j = 0; j < 14; ++j) acc[j] = seg_reduce_to(acc[j], last, lane);
+      if (valid && ((heads >> lane) & 1u)) {
+        double2* H2 = reinterpret_cast<double2*>(P.Hpp + (size_t)pt * 10);
+#pragma unroll
+        for (int j = 0; j < 5; ++j) H2[j] = make_double2(acc[2 * j], acc[2 * j + 1]);
+        double2* G2 = reinterpret_cast<double2*>(P.gp + (size_t)pt * 4);
+        G2[0] = make_double2(acc[10], acc[11]);
+        G2[1] = make_double2(acc[12], acc[13]);
+      }
+    }
+    // camera-side gradient and squared column norms: J_c = [-h Ja | Jw]
+    {
+      const double h = X23.y;
+      double gv[6], cv[6];
+#pragma unroll
+      for (int j = 0; j < 3; ++j) {
+        const double c0 = -h * Ja[j], c1 = -h * Ja[3 + j];
+        gv[j] = c0 * r[0] + c1 * r[1];
+        cv[j] = c0 * c0 + c1 * c1;
+        gv[3 + j] = Jw[j] * r[0] + Jw[3 + j] * r[1];
+        cv[3 + j] = Jw[j] * Jw[j] + Jw[3 + j] * Jw[3 + j];
+      }
+      __syncwarp();  // the previous slice's emission has read the staging rows
+      warp_stage_row<6>(rows, rbase, gv, valid ? cam * 6 : -1, lane);
+      warp_stage_row<6>(rows + 32 * 6, rbase, cv, valid ? cam * 6 : -1, lane);
+      __syncwarp();
+      warp_red_rows<6>(g_cs, rows, rbase, lane);
+      warp_red_rows<6>(cn_cs, rows + 32 * 6, rbase, lane);
+    }
+    if (NI > 0) {
+      if (P.single_group) {
+#pragma unroll
+        for (int j = 0; j < NI; ++j) {
+          gi_acc[j] += Ji[j] * r[0] + Ji[NI + j] * r[1];
+          ci_acc[j] += Ji[j] * Ji[j] + Ji[NI + j] * Ji[NI + j];
+        }
+      } else if (valid) {
+#pragma unroll
+        for (int j = 0; j < NI; ++j) {
+          red_add(g_cs + P.ne + (size_t)grp * 10 + nth_bit(IMASK, j), Ji[j] * r[0] + Ji[NI + j] * r[1]);
+          red_add(cn_cs + P.ne + (size_t)grp * 10 + nth_bit(IMASK, j), Ji[j] * Ji[j] + Ji[NI + j] * Ji[NI + j]);
+        }
+      }
+    }
+    // ---- the stage is consumed: re-arm it for slice s + NS
+    __syncwarp();
+    if (lane == 0 && s + NS < s_end) {
+      fence_proxy_async_smem();  // generic-proxy reads of the stage before the async-proxy refill
+      issue(stage, s + NS);
+    }
+  }
+  // ---- sums that leave the warp once
+  if (s_begin < s_end) {
+    double* rr = rep + (size_t)(gw & (NREP - 1)) * REPW;
+    if (NI > 0 && P.single_group) {
+#pragma unroll
+      for (int j = 0; j < NI; ++j) {
+        const double gsum = warp_sum(gi_acc[j]), csum = warp_sum(ci_acc[j]);
+        if (lane == 0) { red_add(rr + nth_bit(IMASK, j), gsum); red_add(rr + 10 + nth_bit(IMASK, j), csum); }
+      }
+    }
+    const double c = warp_sum(cost_acc), f = warp_sum(fixed_acc), e = warp_sum(failed_acc);
+    if (lane == 0) {
+      red_add(rr + 20, c);
+      if (f != 0.0) red_add(rr + 21, f);
+      if (e != 0.0) red_add(rr + 22, e);
     }
   }
 }

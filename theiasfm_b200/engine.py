@@ -19,7 +19,7 @@ _LIB = None
 # every symbol include/theia_ba_b200.h declares
 EXPORTED_SYMBOLS = [
     "tba_options_init", "tba_device_count", "tba_create", "tba_destroy", "tba_nccl_unique_id", "tba_last_error",
-    "tba_solve", "tba_upload", "tba_minimize", "tba_download", "tba_shard_points", "tba_debug_linearize",
+    "tba_solve", "tba_upload", "tba_minimize", "tba_download", "tba_shard_points", "tba_debug_linearize", "tba_debug_linearize_raw",
     "tba_debug_prepare_linear_system", "tba_debug_schur_matvec", "tba_debug_solve_linear_system",
     "tba_debug_evaluate_step", "tba_debug_read", "tba_reset_parameters", "tba_set_max_iterations", "tba_set_profiling", "tba_get_profile", "tba_get_profile_stages", "tba_solve_multi", "tba_debug_pack", "tba_filter_tracks", "tba_adjust_tracks", "tba_estimate_tracks", "tba_two_view_ba_batch", "tba_two_view_ba_batch_multi",
 ]
@@ -52,6 +52,7 @@ def lib():
         L.tba_download.argtypes = [C.c_void_p, C.POINTER(_abi.tba_problem)]
         L.tba_shard_points.argtypes = [C.POINTER(C.c_int32), C.c_int32, C.c_int, C.c_int, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
         L.tba_debug_linearize.argtypes = [C.c_void_p, dp]
+        L.tba_debug_linearize_raw.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_int64), dp, dp, dp, dp, dp]
         L.tba_debug_prepare_linear_system.argtypes = [C.c_void_p, C.c_double]
         L.tba_debug_schur_matvec.argtypes = [C.c_void_p, dp, dp, dp, dp]
         L.tba_debug_solve_linear_system.argtypes = [C.c_void_p, C.POINTER(C.c_int32), dp]
@@ -314,6 +315,20 @@ class Engine:
         c = C.c_double()
         rc = lib().tba_debug_linearize(self._h, C.byref(c))
         return rc == 0, c.value
+
+    def linearize_raw(self, tile_kernel=False):
+        """tba_debug_linearize_raw: one linearisation; the raw device buffers J [slices, NJ, 32], res [slices, 2, 32], Hpp [n_pt, 10],
+        gp [n_pt, 4] (packed points) and lin = gradient | squared column norms | cost, fixed cost, failed evaluations.
+        tile_kernel: the tile-per-CTA kernel over every tile instead of the streaming kernel over the normal tiles."""
+        sizes = np.zeros(4, np.int64)
+        self._check(lib().tba_debug_linearize_raw(self._h, int(tile_kernel), sizes.ctypes.data_as(C.POINTER(C.c_int64)), None, None, None, None, None))
+        n_slots, nj, n_pt, ncs = (int(v) for v in sizes)
+        J, res = np.zeros((n_slots // 32, nj, 32)), np.zeros((n_slots // 32, 2, 32))
+        Hpp, gp, lin = np.zeros((n_pt, 10)), np.zeros((n_pt, 4)), np.zeros(2 * ncs + 3)
+        self._check(lib().tba_debug_linearize_raw(self._h, int(tile_kernel), sizes.ctypes.data_as(C.POINTER(C.c_int64)),
+                                                  _dp(J), _dp(res), _dp(Hpp), _dp(gp), _dp(lin)))
+        return dict(J=J, res=res, Hpp=Hpp, gp=gp, g=lin[:ncs], cn=lin[ncs:2 * ncs], cost=lin[2 * ncs], fixed=lin[2 * ncs + 1],
+                    failed=lin[2 * ncs + 2])
 
     def prepare_linear_system(self, radius):
         return lib().tba_debug_prepare_linear_system(self._h, radius) == 0
