@@ -345,6 +345,11 @@ int tba_debug_linearize(tba_context* ctx, double* cost);
  * sizes_out = {n_slots, NJ, n_pt, ncs}; with any output pointer NULL only the sizes are returned. */
 int tba_debug_linearize_raw(tba_context* ctx, int tile_kernel, int64_t* sizes_out, double* J, double* res, double* Hpp,
                             double* gp, double* lin);
+/* Launch geometry of the persistent warp-slice kernels over the normal tiles of the uploaded problem (no launch):
+ * out[16] = {n_sm, n_slices, imask, has_ext_models, then {grid, warps per CTA, ring stages} of k_linearize_stream,
+ * k_prepare_stream, k_schur_stream MODE 0 (matvec) and k_schur_stream MODE 1 / 2 (reduced rhs, back-substitution)}.
+ * Warp gw of GW = grid * warps owns the slices [n_slices*gw/GW, n_slices*(gw+1)/GW). */
+int tba_debug_stream_launch(tba_context* ctx, int32_t* out);
 int tba_debug_prepare_linear_system(tba_context* ctx, double radius);
 int tba_debug_schur_matvec(tba_context* ctx, const double* x_cam /*[n_cam*6]*/,
                            const double* x_intr /*[n_group*10]*/,

@@ -24,6 +24,102 @@ def rel_err(a, b):
     return float(np.max(np.abs(a - b)) / max(1e-300, np.max(np.abs(b))))
 
 
+def block_err(a, b, width, floor=None):
+    """Per-block relative error of a against the reference b, blocks of `width` consecutive entries (a camera, a group, a point, an
+    observation): max|a - b| over the block divided by max(max|b_block|, 1e-6 max|b|) -- and by at least floor[block] if given.
+    A block where b is exactly zero must be exactly zero in a as well (constant blocks, masked coordinates), else its error is
+    inf.  Returns (largest error, its block)."""
+    a = np.asarray(a, float).reshape(-1, width); b = np.asarray(b, float).reshape(-1, width)
+    if len(b) == 0:
+        return 0.0, -1
+    d, s = np.abs(a - b).max(axis=1), np.abs(b).max(axis=1)
+    den = np.maximum(s, 1e-6 * s.max() if s.max() > 0 else 1.0)
+    if floor is not None:
+        den = np.maximum(den, floor)
+    err = np.where(s == 0, np.where(np.abs(a).max(axis=1) == 0, 0.0, np.inf), d / den)
+    k = int(np.argmax(err))
+    return float(err[k]), k
+
+
+def warp_slice_counts(n_slices, grid, nw):
+    """Slices per warp of a persistent warp-slice kernel: warp gw of GW = grid * nw owns [n_slices*gw/GW, n_slices*(gw+1)/GW)."""
+    GW = grid * nw
+    return np.diff(n_slices * np.arange(GW + 1, dtype=np.int64) // GW)
+
+
+def cut_tracks(p, lengths, seed=1):
+    """Every track keeps its first n observations, n drawn from `lengths` per point."""
+    target = np.random.default_rng(seed).choice(lengths, size=p.n_pt)
+    order = np.argsort(p.obs_pt, kind="stable")
+    q = p.obs_pt[order]
+    first = np.searchsorted(q, q)  # index of the first observation of the same point in the sorted order
+    keep = np.zeros(p.n_obs, bool)
+    keep[order] = np.arange(p.n_obs) - first < target[q]
+    return _abi.Problem(p.ext, p.ext_const, p.cam_group, p.group_model, p.intr, p.group_const_mask, p.pt, p.pt_const,
+                        p.obs_cam[keep], p.obs_pt[keep], p.obs_xy[keep])
+
+
+STREAM_KERNELS = ("linearize", "prepare", "matvec", "rhs_backsub")
+
+
+def stream_target_slices(geometry, kernel, per_warp):
+    """Normal-tile slice count (a multiple of 8, one tile) giving `kernel` of the launch geometry `geometry` (Engine.stream_launch)
+    per_warp slices in most warps once its grid is capped at one CTA per SM; kernel None: the largest such count over the four.
+    per_warp may be a function of the kernel's ring depth NS."""
+    if kernel is None:
+        return max(stream_target_slices(geometry, k, per_warp) for k in STREAM_KERNELS)
+    if callable(per_warp):
+        per_warp = per_warp(geometry[kernel]["NS"])
+    GW = geometry["n_sm"] * geometry[kernel]["NW"]
+    return max(8, -(-int(round(per_warp * GW)) // 8) * 8)
+
+
+def normal_slices(p):
+    """(slices of the normal tiles, the host packing) of a problem: what the streaming kernels partition among their warps."""
+    from theiasfm_b200 import engine
+    pk = engine.debug_pack(p)
+    assert pk["rc"] == 0, pk["rc"]
+    return 8 * int(((pk["tile_flags"] & 1) == 0).sum()), pk
+
+
+def stream_sized_scene(geometry, kernel, per_warp, extra_slices=0, track_lengths=None, modify=None, **scene_kw):
+    """A seeded synthetic.make_scene(**scene_kw) whose normal tiles hold exactly stream_target_slices(...) + extra_slices warp
+    slices.  The point count is searched with the host packing (engine.debug_pack): tracks are cut to `track_lengths` and
+    `modify(problem)` applied (constant blocks, outliers) before every packing.  Returns (problem, packing)."""
+    from theiasfm_b200 import synthetic
+    target = stream_target_slices(geometry, kernel, per_warp) + extra_slices
+
+    def make(n_pt):
+        p = synthetic.make_scene(n_pt=int(n_pt), **scene_kw)
+        if track_lengths is not None:
+            p = cut_tracks(p, track_lengths)
+        if modify is not None:
+            modify(p)
+        return (p,) + normal_slices(p)
+
+    n_pt, seen = 64, {}
+    lo, hi = 0, None  # n_pt below / above the target
+    for _ in range(60):
+        p, s, pk = make(n_pt)
+        seen[n_pt] = s
+        if s == target:
+            return p, pk
+        if s < target:
+            lo = max(lo, n_pt)
+        else:
+            hi = n_pt if hi is None else min(hi, n_pt)
+        if hi is None:
+            nxt = max(n_pt + 1, int(n_pt * target / max(s, 1) * 1.02))
+        elif hi - lo <= 1:
+            break
+        else:  # interpolate inside the bracket, never on its ends
+            s_lo = seen.get(lo, 0)
+            nxt = lo + int(round((hi - lo) * (target - s_lo) / max(seen[hi] - s_lo, 1)))
+            nxt = min(max(nxt, lo + 1), hi - 1)
+        n_pt = nxt
+    raise AssertionError("no point count packs to %d normal slices (tried %s)" % (target, sorted(seen.items())))
+
+
 def free_masks(p):
     """(free_cam [n_cam,6], free_intr [n_group,10], free_pt [n_pt,4]) booleans."""
     fc = np.ones((p.n_cam, 6), bool)

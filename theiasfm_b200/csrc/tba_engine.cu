@@ -265,6 +265,9 @@ double* lin_scal(tba_context* c) { return c->lin.p + 2 * (size_t)c->P.ncs; }
 // grid of the per-point / per-element streaming kernels (256 threads per CTA): enough CTAs to cover the latency of a dependent
 // load chain (8 per SM), not more than the work
 int small_grid(const tba_context* c, int64_t n_items) { return (int)std::max<int64_t>(1, std::min<int64_t>((n_items + 255) / 256, (int64_t)c->n_sm * 8)); }
+// grid of the persistent warp-slice kernels (k_linearize_stream, k_prepare_stream, k_schur_stream) with NW warps per CTA: at most
+// one CTA per SM, and no more warps than slices; warp gw of the GW = grid * NW owns slices [n_slices*gw/GW, n_slices*(gw+1)/GW)
+int stream_grid(const tba_context* c, int n_slices, int NW) { return std::max(1, std::min(c->n_sm, (n_slices + NW - 1) / NW)); }
 
 // scal layout: 0 cost, 1 fixed cost, 2 failed evals, 3 model cost change, 4 |delta_cs|^2, 5 |delta_pt|^2,
 //              6 |x_cs|^2, 7 |x_pt|^2
@@ -296,7 +299,7 @@ int stage_linearize(tba_context* c, double* cost, double* fixed, bool* ok, doubl
       if (c->n_normal_tiles > 0 && !tile_kernel) {
         const int n_slices = c->n_normal_tiles * (TILE / 32);
 #define F(M) { using Cfg = LinCfg<M>; auto kfn = k_linearize_stream<M>; \
-               const int grid = std::max(1, std::min(c->n_sm, (n_slices + Cfg::NW - 1) / Cfg::NW)); \
+               const int grid = stream_grid(c, n_slices, Cfg::NW); \
                LAUNCH(c, kfn, grid, Cfg::NW * 32, Cfg::SMEM, P, lin_g(c), lin_cn(c), c->rep.p, n_slices); }
         DISPATCH_IMASK(c->imask, F)
 #undef F
@@ -443,7 +446,7 @@ int launch_schur(tba_context* c, const double* xs, double* y, const int* done, c
   if (c->n_normal_tiles > 0) {
     const int n_slices = c->n_normal_tiles * (TILE / 32);
 #define F(M) { using Cfg = StreamCfg<M, MODE>; auto kfn = k_schur_stream<M, MODE>; \
-               const int grid = std::max(1, std::min(c->n_sm, (n_slices + Cfg::NW - 1) / Cfg::NW)); \
+               const int grid = stream_grid(c, n_slices, Cfg::NW); \
                LAUNCH(c, kfn, grid, Cfg::NW * 32, Cfg::SMEM, P, xs, y, c->rep.p, done, n_slices, pp); }
     DISPATCH_IMASK(c->imask, F)
 #undef F
@@ -483,7 +486,7 @@ int stage_prepare(tba_context* c, double radius, bool* ok, bool defer_flag = fal
       const int n_slices = c->n_normal_tiles * (TILE / 32);
       const int pb = prof_begin(c);
 #define F(M) { using Cfg = PrepCfg<M>; auto kfn = k_prepare_stream<M>; \
-               const int grid = std::max(1, std::min(c->n_sm, (n_slices + Cfg::NW - 1) / Cfg::NW)); \
+               const int grid = stream_grid(c, n_slices, Cfg::NW); \
                LAUNCH(c, kfn, grid, Cfg::NW * 32, Cfg::SMEM, P, yr, c->Sblk.p, c->Sblk.p + (size_t)P.n_cam * 21, c->rep.p, n_slices); }
       DISPATCH_IMASK(c->imask, F)
 #undef F
@@ -1964,6 +1967,18 @@ int tba_debug_linearize_raw(tba_context* c, int tile_kernel, int64_t* sizes_out,
   CUDA_OK(c, cudaMemcpyAsync(gp, P.gp, (size_t)P.n_pt * 4 * 8, cudaMemcpyDeviceToHost, c->stream));
   CUDA_OK(c, cudaMemcpyAsync(lin, c->lin.p, (2 * (size_t)P.ncs + 3) * 8, cudaMemcpyDeviceToHost, c->stream));
   CUDA_OK(c, cudaStreamSynchronize(c->stream));
+  return TBA_OK;
+}
+
+int tba_debug_stream_launch(tba_context* c, int32_t* out) {
+  if (!c || !c->uploaded || !out) return TBA_ERR_INVALID_ARGUMENT;
+  const int n_slices = c->n_normal_tiles * (TILE / 32);
+  out[0] = c->n_sm; out[1] = n_slices; out[2] = (int32_t)c->imask; out[3] = c->has_ext_models ? 1 : 0;
+  auto put = [&](int k, int NW, int NS) { out[4 + 3 * k] = stream_grid(c, n_slices, NW); out[5 + 3 * k] = NW; out[6 + 3 * k] = NS; };
+#define F(M) { put(0, LinCfg<M>::NW, LinCfg<M>::NS); put(1, PrepCfg<M>::NW, PrepCfg<M>::NS); \
+               put(2, StreamCfg<M, 0>::NW, StreamCfg<M, 0>::NS); put(3, StreamCfg<M, 1>::NW, StreamCfg<M, 1>::NS); }
+  DISPATCH_IMASK(c->imask, F)
+#undef F
   return TBA_OK;
 }
 

@@ -20,6 +20,7 @@ _LIB = None
 EXPORTED_SYMBOLS = [
     "tba_options_init", "tba_device_count", "tba_create", "tba_destroy", "tba_nccl_unique_id", "tba_last_error",
     "tba_solve", "tba_upload", "tba_minimize", "tba_download", "tba_shard_points", "tba_debug_linearize", "tba_debug_linearize_raw",
+    "tba_debug_stream_launch",
     "tba_debug_prepare_linear_system", "tba_debug_schur_matvec", "tba_debug_solve_linear_system",
     "tba_debug_evaluate_step", "tba_debug_read", "tba_reset_parameters", "tba_set_max_iterations", "tba_set_profiling", "tba_get_profile", "tba_get_profile_stages", "tba_solve_multi", "tba_debug_pack", "tba_filter_tracks", "tba_adjust_tracks", "tba_estimate_tracks", "tba_two_view_ba_batch", "tba_two_view_ba_batch_multi",
 ]
@@ -53,6 +54,7 @@ def lib():
         L.tba_shard_points.argtypes = [C.POINTER(C.c_int32), C.c_int32, C.c_int, C.c_int, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
         L.tba_debug_linearize.argtypes = [C.c_void_p, dp]
         L.tba_debug_linearize_raw.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_int64), dp, dp, dp, dp, dp]
+        L.tba_debug_stream_launch.argtypes = [C.c_void_p, C.POINTER(C.c_int32)]
         L.tba_debug_prepare_linear_system.argtypes = [C.c_void_p, C.c_double]
         L.tba_debug_schur_matvec.argtypes = [C.c_void_p, dp, dp, dp, dp]
         L.tba_debug_solve_linear_system.argtypes = [C.c_void_p, C.POINTER(C.c_int32), dp]
@@ -329,6 +331,19 @@ class Engine:
                                                   _dp(J), _dp(res), _dp(Hpp), _dp(gp), _dp(lin)))
         return dict(J=J, res=res, Hpp=Hpp, gp=gp, g=lin[:ncs], cn=lin[ncs:2 * ncs], cost=lin[2 * ncs], fixed=lin[2 * ncs + 1],
                     failed=lin[2 * ncs + 2])
+
+    STREAM_KERNELS = ("linearize", "prepare", "matvec", "rhs_backsub")
+
+    def stream_launch(self):
+        """tba_debug_stream_launch: the launch geometry of the persistent warp-slice kernels over the uploaded normal tiles.
+        {n_sm, n_slices, imask, has_ext_models, and per kernel in STREAM_KERNELS: {grid, NW, NS}}; k_linearize_stream,
+        k_prepare_stream, k_schur_stream MODE 0 and MODE 1 / 2.  Warp gw of GW = grid * NW owns [n_slices*gw/GW, n_slices*(gw+1)/GW)."""
+        out = np.zeros(16, np.int32)
+        self._check(lib().tba_debug_stream_launch(self._h, out.ctypes.data_as(C.POINTER(C.c_int32))))
+        d = dict(n_sm=int(out[0]), n_slices=int(out[1]), imask=int(out[2]), has_ext_models=bool(out[3]))
+        for k, name in enumerate(self.STREAM_KERNELS):
+            d[name] = dict(grid=int(out[4 + 3 * k]), NW=int(out[5 + 3 * k]), NS=int(out[6 + 3 * k]))
+        return d
 
     def prepare_linear_system(self, radius):
         return lib().tba_debug_prepare_linear_system(self._h, radius) == 0
