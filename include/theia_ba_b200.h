@@ -258,6 +258,24 @@ enum { TBA_TRACK_ESTIMATED = 0, TBA_TRACK_BAD_ANGLE = 1, TBA_TRACK_TRIANGULATION
        TBA_TRACK_BAD_REPROJECTION = 4, TBA_TRACK_SKIPPED = 255 };
 
 /*
+ * N3: BundleAdjustView (src/theia/sfm/bundle_adjustment/bundle_adjustment.cc:83-93, DENSE_QR, no inner iterations) for every
+ * camera views[0..n_views) of the uploaded problem at once -- what LocalizeViewToReconstruction runs last for each newly
+ * localized view (localize_view_to_reconstruction.cc:246-252).  Per view: one reprojection residual per observation of that
+ * camera, every point constant, the free parameters are the camera's extrinsics and its intrinsics group with the coordinates
+ * ext_const / group_const_mask of the upload leave free (at most 6 + 10).  options: loss and width, max_num_iterations,
+ * tolerances and trust-region fields of tba_options; linear_solver_type and use_inner_iterations are ignored.  A view without
+ * observations or without a free coordinate converges at iteration 0, parameters untouched, initial = final cost = its cost.
+ * status[v]: TBA_CONVERGENCE / NO_CONVERGENCE / FAILURE (BundleAdjustmentSummary::success = status != TBA_FAILURE);
+ * initial_cost / final_cost / iterations: optional, [n_views] (-1 costs where the initial evaluation failed).
+ * Read the refined ext / intr back with tba_download; nothing else changes.
+ * TBA_ERR_INVALID_ARGUMENT, with nothing changed: a view index out of range or listed twice, or two views that share an
+ * intrinsics group with a free coordinate (one call per view would see the previous call's intrinsics -- adjust such views in
+ * separate calls).  TBA_ERR_UNSUPPORTED on a context of a multi-rank group.
+ */
+int tba_adjust_views(tba_context* ctx, const tba_options* options, const int32_t* views, int32_t n_views, uint8_t* status,
+                     double* initial_cost, double* final_cost, int32_t* iterations);
+
+/*
  * N3: BundleAdjustTwoViews (src/theia/sfm/bundle_adjustment/bundle_adjust_two_views.cc:112-191) for MANY image pairs in one
  * call -- what TwoViewMatchGeometricVerification issues once per pair (two_view_match_geometric_verification.cc:268-296).
  * Per pair: camera 1 fixed, camera 2's extrinsics free, each camera's intrinsics constant or focal-length-only, every point

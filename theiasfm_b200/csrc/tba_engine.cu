@@ -146,6 +146,15 @@ struct tba_context {
   DevBuf<double> d_blk_vals, d_blk_rec, d_blk_acc, d_inner_cost2;
   DevBuf<uint8_t> d_inner_status;
   int64_t inner_passes = 0;
+  std::vector<int> h_cam_group;
+  // camera-major index of the uploaded observation slots (tba_adjust_views): camera c owns cam_slot[cam_off[c] .. cam_off[c+1]),
+  // in ascending slot order; built on first use after an upload
+  bool cam_index_ready = false;
+  DevBuf<long long> cam_off, cam_slot;
+  DevBuf<int> view_cam, view_it;        // per-view inputs / outputs of tba_adjust_views (grown, never shrunk)
+  DevBuf<uint32_t> view_fm;
+  DevBuf<uint8_t> view_status;
+  DevBuf<double> view_cost2;
   bool has_ext_models = false;  // some group uses FISHEYE / FOV / DIVISION_UNDISTORTION: EXT kernel instantiations
   double trace_pcg_gpu_ms = 0.0;  // TBA_TRACE_LM: device-side span of the PCG launches (first launch .. state copy), summed over a minimize
   int n_normal_tiles = 0;   // tiles whose tracks fit a warp slice (they precede the long tiles)
@@ -1250,10 +1259,12 @@ int tba_upload(tba_context* c, const tba_options* options, const tba_problem* p)
     }
   }
   c->have_scale = false;
+  c->h_ext_const.assign(p->ext_const, p->ext_const + nc);
+  c->h_group_mask.assign(p->group_const_mask, p->group_const_mask + ng);
+  c->h_group_model.assign(p->group_model, p->group_model + ng);
+  c->h_cam_group.assign(p->cam_group, p->cam_group + nc);
+  c->cam_index_ready = false;
   if (c->opt.use_inner_iterations) {
-    c->h_ext_const.assign(p->ext_const, p->ext_const + nc);
-    c->h_group_mask.assign(p->group_const_mask, p->group_const_mask + ng);
-    c->h_group_model.assign(p->group_model, p->group_model + ng);
     CUDA_OK(c, c->d_ext_const.alloc((size_t)nc)); CUDA_OK(c, c->d_group_mask.alloc((size_t)ng));
     // every buffer the inner iterations use is allocated here, never inside tba_minimize (no cudaMalloc between collectives)
     CUDA_OK(c, c->d_blk_vals.alloc(std::max((size_t)nc * 6, (size_t)ng * 10)));
@@ -1668,6 +1679,107 @@ int tba_estimate_tracks(tba_context* c, const tba_options* ba_options, double ma
     for (int j = 0; j < 5; ++j) counts[j] = 0;
     for (int q = 0; q < c->n_pt_caller; ++q)
       if (status[q] < 5) ++counts[status[q]];
+  }
+  return TBA_OK;
+}
+
+// --------------------------------------------------------------------------- N3: batched BundleAdjustView
+namespace {
+// Counting sort of the packed observation slots by camera (ascending slot order inside a camera), from the device's slot_cam.
+int build_cam_index(tba_context* c) {
+  const int nc = c->n_cam;
+  const int64_t ns = c->n_slots;
+  std::vector<int> sc((size_t)ns);
+  if (ns > 0) {
+    CUDA_OK(c, cudaMemcpyAsync(sc.data(), c->slot_cam.p, (size_t)ns * 4, cudaMemcpyDeviceToHost, c->stream));
+    CUDA_OK(c, cudaStreamSynchronize(c->stream));
+  }
+  std::vector<long long> off((size_t)nc + 1, 0);
+  for (int64_t s = 0; s < ns; ++s) if (sc[s] >= 0) ++off[(size_t)sc[s] + 1];
+  for (int i = 0; i < nc; ++i) off[(size_t)i + 1] += off[i];
+  std::vector<long long> cur(off.begin(), off.end() - 1), slot((size_t)std::max<long long>(off[nc], 1));
+  for (int64_t s = 0; s < ns; ++s) if (sc[s] >= 0) slot[(size_t)cur[sc[s]]++] = (long long)s;
+  CUDA_OK(c, c->cam_off.alloc(off.size()));
+  CUDA_OK(c, c->cam_slot.alloc(slot.size()));
+  CUDA_OK(c, cudaMemcpyAsync(c->cam_off.p, off.data(), off.size() * 8, cudaMemcpyHostToDevice, c->stream));
+  CUDA_OK(c, cudaMemcpyAsync(c->cam_slot.p, slot.data(), slot.size() * 8, cudaMemcpyHostToDevice, c->stream));
+  CUDA_OK(c, cudaStreamSynchronize(c->stream));
+  c->d2h_bytes += (double)ns * 4; c->h2d_bytes += (double)(off.size() + slot.size()) * 8;
+  c->cam_index_ready = true;
+  return TBA_OK;
+}
+}  // namespace
+
+int tba_adjust_views(tba_context* c, const tba_options* options, const int32_t* views, int32_t n_views, uint8_t* status, double* initial_cost,
+                     double* final_cost, int32_t* iterations) {
+  if (!c || !c->uploaded || !options || n_views < 0 || (n_views > 0 && !views)) return TBA_ERR_INVALID_ARGUMENT;
+  if (c->world > 1) { set_err(c, "tba_adjust_views runs on a single-rank context (the views' observations must all be on this device)"); return TBA_ERR_UNSUPPORTED; }
+  if (options->loss_function_type < 0 || options->loss_function_type > 5) { set_err(c, "invalid loss function type %d", options->loss_function_type); return TBA_ERR_INVALID_ARGUMENT; }
+  const int nc = c->n_cam, ng = c->n_group;
+  // validate the whole batch before anything changes: indices, duplicates, intrinsics groups with a free coordinate that two views
+  // of the batch share (sequential BundleAdjustView calls would each see the previous call's intrinsics: not batchable)
+  std::vector<uint32_t> fm((size_t)n_views);
+  std::vector<int> seen((size_t)nc, -1), group_view((size_t)ng, -1);
+  for (int v = 0; v < n_views; ++v) {
+    const int cam = views[v];
+    if (cam < 0 || cam >= nc) { set_err(c, "views[%d] = %d is not a camera index (0..%d)", v, cam, nc - 1); return TBA_ERR_INVALID_ARGUMENT; }
+    if (seen[cam] >= 0) { set_err(c, "camera %d is listed twice (views[%d] and views[%d])", cam, seen[cam], v); return TBA_ERR_INVALID_ARGUMENT; }
+    seen[cam] = v;
+    const int g = c->h_cam_group[cam], K = TBA_MODEL_NUM_PARAMETERS(c->h_group_model[g]);
+    uint32_t m = 0;
+    const uint8_t ec = c->h_ext_const[cam];
+    if (!(ec & TBA_EXT_POSITION_CONST)) m |= 0x7u;
+    if (!(ec & TBA_EXT_ORIENTATION_CONST)) m |= 0x38u;
+    for (int j = 0; j < K; ++j) if (!((c->h_group_mask[g] >> j) & 1u)) m |= 1u << (6 + j);
+    fm[v] = m;
+    if (m & 0xFFC0u) {
+      if (group_view[g] >= 0) {
+        set_err(c, "views[%d] (camera %d) and views[%d] (camera %d) share intrinsics group %d, which has free coordinates: one call per view would "
+                   "see the previous call's intrinsics, so they cannot be adjusted in one batch", group_view[g], views[group_view[g]], v, cam, g);
+        return TBA_ERR_INVALID_ARGUMENT;
+      }
+      group_view[g] = v;
+    }
+  }
+  if (n_views == 0) return TBA_OK;
+  CUDA_OK(c, cudaSetDevice(c->device));
+  if (!c->cam_index_ready) {
+    const int rc = build_cam_index(c);
+    if (rc) return rc;
+  }
+  DevBuf<int>& d_cam = c->view_cam;
+  DevBuf<int>& d_it = c->view_it;
+  DevBuf<uint32_t>& d_fm = c->view_fm;
+  DevBuf<uint8_t>& d_status = c->view_status;
+  DevBuf<double>& d_cost2 = c->view_cost2;
+  CUDA_OK(c, d_cam.alloc((size_t)n_views)); CUDA_OK(c, d_fm.alloc((size_t)n_views)); CUDA_OK(c, d_it.alloc((size_t)n_views));
+  CUDA_OK(c, d_status.alloc((size_t)n_views)); CUDA_OK(c, d_cost2.alloc((size_t)n_views * 2));
+  CUDA_OK(c, cudaMemcpyAsync(d_cam.p, views, (size_t)n_views * 4, cudaMemcpyHostToDevice, c->stream));
+  CUDA_OK(c, cudaMemcpyAsync(d_fm.p, fm.data(), (size_t)n_views * 4, cudaMemcpyHostToDevice, c->stream));
+  c->h2d_bytes += (double)n_views * 8;
+  DevProblem& P = c->P;
+  ViewBatchDev B;
+  B.n_views = n_views; B.cam = d_cam.p; B.free_mask = d_fm.p; B.cam_off = c->cam_off.p; B.cam_slot = c->cam_slot.p;
+  B.ext = P.ext; B.intr = P.intr; B.cam_group = P.cam_group; B.group_model = P.group_model; B.slot_pt = P.slot_pt; B.pt = P.pt; B.xy = P.xy;
+  {
+    auto kfn = c->has_ext_models ? k_view_ba<true> : k_view_ba<false>;
+    LAUNCH(c, kfn, (unsigned)n_views, kViewThreads, 0, B, point_lm_options(*options), d_status.p, d_cost2.p, d_it.p);
+  }
+  // the rotation records of the adjusted cameras, for the passes that read them (tba_minimize, the track stages)
+  LAUNCH(c, k_cam_prep, (nc + 127) / 128, 128, 0, nc, P.ext, P.cam_rec, P.cam_s4);
+  std::vector<double> hc((size_t)n_views * 2);
+  std::vector<uint8_t> hs((size_t)n_views);
+  std::vector<int> hit((size_t)n_views);
+  CUDA_OK(c, cudaMemcpyAsync(hs.data(), d_status.p, (size_t)n_views, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_OK(c, cudaMemcpyAsync(hc.data(), d_cost2.p, (size_t)n_views * 16, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_OK(c, cudaMemcpyAsync(hit.data(), d_it.p, (size_t)n_views * 4, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_OK(c, cudaStreamSynchronize(c->stream));
+  c->d2h_bytes += (double)n_views * 21;
+  for (int v = 0; v < n_views; ++v) {
+    if (status) status[v] = hs[v];
+    if (initial_cost) initial_cost[v] = hc[(size_t)2 * v];
+    if (final_cost) final_cost[v] = hc[(size_t)2 * v + 1];
+    if (iterations) iterations[v] = hit[v];
   }
   return TBA_OK;
 }

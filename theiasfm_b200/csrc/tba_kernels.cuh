@@ -14,6 +14,7 @@
 #include "tba_filter.cuh"
 #include "tba_track_estimator.cuh"
 #include "tba_two_view.cuh"
+#include "tba_view_ba.cuh"
 
 namespace tba {
 

@@ -47,6 +47,7 @@ struct SerialTeam {
   __host__ __device__ static double sum(double v) { return v; }
   __host__ __device__ static double max(double v) { return v; }
   __host__ __device__ static bool all(bool v) { return v; }
+  __host__ __device__ static void sync() {}
 };
 struct WarpTeam {
   __host__ __device__ static int rank() {

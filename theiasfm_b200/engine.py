@@ -22,7 +22,7 @@ EXPORTED_SYMBOLS = [
     "tba_solve", "tba_upload", "tba_minimize", "tba_download", "tba_shard_points", "tba_debug_linearize", "tba_debug_linearize_raw",
     "tba_debug_stream_launch",
     "tba_debug_prepare_linear_system", "tba_debug_schur_matvec", "tba_debug_solve_linear_system",
-    "tba_debug_evaluate_step", "tba_debug_read", "tba_reset_parameters", "tba_set_max_iterations", "tba_set_profiling", "tba_get_profile", "tba_get_profile_stages", "tba_solve_multi", "tba_debug_pack", "tba_filter_tracks", "tba_adjust_tracks", "tba_estimate_tracks", "tba_two_view_ba_batch", "tba_two_view_ba_batch_multi",
+    "tba_debug_evaluate_step", "tba_debug_read", "tba_reset_parameters", "tba_set_max_iterations", "tba_set_profiling", "tba_get_profile", "tba_get_profile_stages", "tba_solve_multi", "tba_debug_pack", "tba_filter_tracks", "tba_adjust_tracks", "tba_adjust_views", "tba_estimate_tracks", "tba_two_view_ba_batch", "tba_two_view_ba_batch_multi",
 ]
 
 
@@ -64,6 +64,8 @@ def lib():
         L.tba_solve_multi.argtypes = [C.POINTER(_abi.tba_options), C.POINTER(_abi.tba_problem), C.POINTER(_abi.tba_summary), C.c_int]
         L.tba_debug_pack.restype = C.c_int
         L.tba_adjust_tracks.argtypes = [C.c_void_p, C.POINTER(_abi.tba_options), C.POINTER(C.c_uint8), dp, dp, C.POINTER(C.c_int32)]
+        L.tba_adjust_views.argtypes = [C.c_void_p, C.POINTER(_abi.tba_options), C.POINTER(C.c_int32), C.c_int32, C.POINTER(C.c_uint8), dp, dp,
+                                       C.POINTER(C.c_int32)]
         L.tba_estimate_tracks.argtypes = [C.c_void_p, C.POINTER(_abi.tba_options), C.c_double, C.c_double, C.c_int32, C.POINTER(C.c_uint8), C.POINTER(C.c_int32)]
         L.tba_two_view_ba_batch_multi.argtypes = [C.POINTER(_abi.tba_two_view_batch), C.c_int, C.POINTER(C.c_uint8), dp, dp, C.POINTER(C.c_int32)]
         L.tba_two_view_ba_batch.argtypes = [C.c_void_p, C.POINTER(_abi.tba_two_view_batch), C.POINTER(C.c_uint8), dp, dp, C.POINTER(C.c_int32)]
@@ -268,6 +270,16 @@ class Engine:
         self._check(lib().tba_adjust_tracks(self._h, C.byref(options), status.ctypes.data_as(C.POINTER(C.c_uint8)), _dp(ic), _dp(fc), C.byref(nf)))
         n = self._problem.n_pt
         return status[:n], ic[:n], fc[:n], nf.value
+
+    def adjust_views(self, options, views):
+        """tba_adjust_views (batched BundleAdjustView) on the device-resident problem for the cameras `views`; call download() for
+        the refined extrinsics and intrinsics.  Returns (status [n] uint8, initial_cost [n], final_cost [n], iterations [n] int32)."""
+        v = np.ascontiguousarray(views, dtype=np.int32).reshape(-1)
+        n = len(v)
+        status = np.zeros(max(n, 1), np.uint8); ic = np.zeros(max(n, 1)); fc = np.zeros(max(n, 1)); it = np.zeros(max(n, 1), np.int32)
+        self._check(lib().tba_adjust_views(self._h, C.byref(options), v.ctypes.data_as(C.POINTER(C.c_int32)), n,
+                                           status.ctypes.data_as(C.POINTER(C.c_uint8)), _dp(ic), _dp(fc), it.ctypes.data_as(C.POINTER(C.c_int32))))
+        return status[:n], ic[:n], fc[:n], it[:n]
 
     def estimate_tracks(self, options, max_reprojection_error_pixels=5.0, min_triangulation_angle_degrees=3.0, bundle_adjustment=True):
         """tba_estimate_tracks (batched TrackEstimator::EstimateTrack); call download() for the points. Returns (status, counts[5])."""
