@@ -59,6 +59,56 @@ def cut_tracks(p, lengths, seed=1):
                         p.obs_cam[keep], p.obs_pt[keep], p.obs_xy[keep])
 
 
+def exact_tracks(p, lengths):
+    """Point i of the result is a track of exactly lengths[i] observations: the first lengths[i] observations of the next point
+    of p, in caller order, that has at least that many.  Long tracks are packed into long tiles in caller order, so the list
+    fixes the long-tile layout."""
+    order = np.argsort(p.obs_pt, kind="stable")
+    counts = np.bincount(p.obs_pt, minlength=p.n_pt)
+    begin = np.concatenate([[0], np.cumsum(counts)])
+    src, q = [], 0
+    for n in lengths:
+        while q < p.n_pt and counts[q] < n:
+            q += 1
+        assert q < p.n_pt, "the scene has too few points with %d observations" % n
+        src.append(q)
+        q += 1
+    idx = np.concatenate([order[begin[q]:begin[q] + n] for q, n in zip(src, lengths)])
+    return _abi.Problem(p.ext, p.ext_const, p.cam_group, p.group_model, p.intr, p.group_const_mask, p.pt[src], p.pt_const[src],
+                        p.obs_cam[idx], np.repeat(np.arange(len(lengths), dtype=np.int32), lengths), p.obs_xy[idx])
+
+
+# Long tracks in caller order and the long tiles they pack into (tile-relative slot ranges):
+#   [0, 256)                                   one point fills the tile
+#   [0, 255) + padding                         the largest point that leaves a padding slot
+#   [0, 33) [33, 133) [133, 197)               a point from lane 1 of slice 1 over slices 1..4
+#   [0, 96) [96, 129)                          ends on a warp boundary / one slot past one
+#   [0, 128) [128, 256)
+#   [0, 64) [64, 97) [97, 247)
+#   [0, 65) [65, 255)
+#   seven points of 36
+LONG_LAYOUT = (256, 255, 33, 100, 64, 96, 33, 128, 128, 64, 33, 150, 65, 190) + (36,) * 7
+
+
+def long_track_scene(seed, filler=24, short=0, n_cam=260, **scene_kw):
+    """synthetic.make_scene(n_cam, seed=seed, **scene_kw) cut to the tracks LONG_LAYOUT, then `filler` more tracks of 33..256
+    observations and `short` tracks of 2..32 (normal tiles), in that caller order.  A 256-observation track needs 256 cameras."""
+    rng = np.random.default_rng(seed)
+    lengths = list(LONG_LAYOUT) + rng.integers(33, 257, filler).tolist() + rng.integers(2, 33, short).tolist()
+    from theiasfm_b200 import synthetic
+    p = synthetic.make_scene(n_cam=n_cam, n_pt=len(lengths) + 40, obs_per_pt=256, seed=seed, **scene_kw)
+    return exact_tracks(p, lengths)
+
+
+def packed_extents(pk):
+    """(tile, first slot inside the tile, observation count) of every packed point of the host packing pk (engine.debug_pack)."""
+    valid = pk["slot_cam"] >= 0
+    slots, kp = np.nonzero(valid)[0], pk["slot_pt"][valid]
+    first = np.zeros(pk["n_packed_points"], np.int64)
+    first[kp[::-1]] = slots[::-1]
+    return first // 256, first % 256, np.bincount(kp, minlength=pk["n_packed_points"])
+
+
 STREAM_KERNELS = ("linearize", "prepare", "matvec", "rhs_backsub")
 
 

@@ -4,6 +4,7 @@ long tracks live in long tiles, runs / flags / masks follow the rules of DESIGN.
 import numpy as np
 import pytest
 
+from helpers import exact_tracks
 from theiasfm_b200 import _abi, engine, synthetic
 
 
@@ -31,9 +32,34 @@ def _ragged_scene(seed=3, n_groups_mode="shared"):
     return q
 
 
-@pytest.mark.parametrize("mode", ["shared", "per_camera", "few"])
+LONG_TRACKS = {
+    "track_256": [256],                 # 256 per-camera groups: 256 runs, the most a point (and a tile) can have
+    "track_256_repeat": [256],          # the same track with one camera observing the point twice: 255 runs
+    "track_255": [255],                 # a padding slot behind it
+    "long_33_36": [33] * 7 + [36] * 7,  # two long tiles of seven points each
+}
+
+
+def _long_scene(mode, seed=7):
+    """Long tracks over per-camera intrinsics groups (a point has one run per distinct camera), a few short ones, observations in
+    random order."""
+    lengths = LONG_TRACKS[mode] + [2, 9, 32]
+    p = synthetic.make_scene(n_cam=260, n_pt=len(lengths) + 8, obs_per_pt=max(lengths), seed=seed, shared_intrinsics=False)
+    p = exact_tracks(p, lengths)
+    if mode == "track_256_repeat":
+        o = np.nonzero(p.obs_pt == 0)[0]
+        p.obs_cam[o[100]] = p.obs_cam[o[7]]
+    perm = np.random.default_rng(seed).permutation(p.n_obs)
+    q = _abi.Problem(p.ext, p.ext_const, p.cam_group, p.group_model, p.intr, p.group_const_mask, p.pt, p.pt_const,
+                     p.obs_cam[perm], p.obs_pt[perm], p.obs_xy[perm])
+    q.ext_const[5] = _abi.EXT_ALL_CONST
+    q.pt_const[[1, len(lengths) - 1]] = 1
+    return q
+
+
+@pytest.mark.parametrize("mode", ["shared", "per_camera", "few"] + list(LONG_TRACKS))
 def test_pack_invariants(mode):
-    p = _ragged_scene(seed=7, n_groups_mode=mode)
+    p = _long_scene(mode) if mode in LONG_TRACKS else _ragged_scene(seed=7, n_groups_mode=mode)
     k = engine.debug_pack(p)
     assert k["rc"] == 0
     n_slots, n_tiles = k["n_slots"], k["n_tiles"]
@@ -57,7 +83,7 @@ def test_pack_invariants(mode):
     assert np.array_equal(pk[:n_short], np.nonzero((counts > 0) & (counts <= 32))[0])
     assert np.array_equal(pk[n_short:], np.nonzero(counts > 32)[0]) and k["n_long_points"] == int((counts > 32).sum())
     # 3. per packed point: contiguous slots, inside one tile; short tracks inside one warp slice of a normal tile,
-    #    long tracks in long tiles; (group, camera) order inside the point
+    #    long tracks in long tiles; (group, camera, observation index) order inside the point
     tb = k["tile_pt_begin"]
     assert tb[0] == 0 and tb[-1] == len(pk) and (np.diff(tb) > 0).all() and (np.diff(tb) <= 256).all()
     for kp in range(len(pk)):
@@ -70,8 +96,8 @@ def test_pack_invariants(mode):
         else:
             assert k["tile_flags"][t] == 1
         cams = k["slot_cam"][sl]
-        key = p.cam_group[cams].astype(np.int64) * 100000 + cams
-        assert (np.diff(key) > 0).all()
+        key = np.diff(p.cam_group[cams].astype(np.int64) * 100000 + cams)
+        assert ((key > 0) | ((key == 0) & (np.diff(k["slot_orig"][sl]) > 0))).all()
     # 4. runs: a new run whenever (point, group) changes, numbered from 0 inside each tile
     for t in range(n_tiles):
         sl = np.arange(t * 256, (t + 1) * 256)

@@ -3,7 +3,7 @@ restatement on the parameters the solve returned.  First executed by the round-e
 import numpy as np
 import pytest
 
-from helpers import fountain_problem
+from helpers import fountain_problem, long_track_scene
 from theiasfm_b200 import _abi, engine, synthetic
 
 pytestmark = pytest.mark.gpu
@@ -13,6 +13,7 @@ KW = dict(use_inner_iterations=0, linear_solver_type=_abi.ITERATIVE_SCHUR, max_n
 def _check(eng, oracle, p, thresholds):
     s = eng.solve(p, engine.default_options(**KW))   # p now holds the refined parameters; the device copy is resident
     assert s.rc == 0
+    statuses = []
     for max_err, angle in thresholds:
         st, mean, nb, ni = eng.filter_tracks(max_err, angle)
         st_o, mean_o, removed = oracle.filter_tracks(p, max_err, angle)
@@ -22,6 +23,8 @@ def _check(eng, oracle, p, thresholds):
         borderline = ok & (np.abs(mean_o - max_err ** 2) <= 1e-9 * max_err ** 2)
         assert np.array_equal(st[~borderline], st_o[~borderline])
         assert abs((nb + ni) - removed) <= int(borderline.sum())
+        statuses.append(st_o)
+    return np.concatenate(statuses)
 
 
 def test_filter_matches_oracle_on_synthetic_with_outliers(oracle):
@@ -32,6 +35,18 @@ def test_filter_matches_oracle_on_synthetic_with_outliers(oracle):
     eng = engine.Engine()
     _check(eng, oracle, p, [(5.0, 3.0), (1.0, 1.0), (0.6, 20.0)])
     eng.close()
+
+
+def test_filter_matches_oracle_on_long_tracks(oracle):
+    """Tracks of 33..256 observations (helpers.long_track_scene): k_filter_tracks walks each one over the warp slices of a long
+    tile, from mid-warp starts and across padding.  The thresholds give all three outcomes."""
+    p = long_track_scene(seed=14, filler=40)
+    rng = np.random.default_rng(3)
+    p.obs_xy[rng.choice(p.n_obs, 40, replace=False)] += 30.0
+    eng = engine.Engine()
+    st = _check(eng, oracle, p, [(5.0, 3.0), (3.0, 1.0), (5.0, 60.0)])
+    eng.close()
+    assert set(np.unique(st).tolist()) == {0, 1, 2}
 
 
 def test_filter_on_the_reference_fountain_reconstruction(oracle):

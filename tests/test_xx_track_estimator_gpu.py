@@ -5,7 +5,7 @@ the upload / download glue and the packed <-> caller scatter.  Never executed on
 import numpy as np
 import pytest
 
-from helpers import fountain_problem
+from helpers import fountain_problem, long_track_scene
 from theiasfm_b200 import _abi, engine, synthetic
 
 pytestmark = pytest.mark.gpu
@@ -24,6 +24,25 @@ def test_estimate_tracks_matches_oracle(oracle, model, ba):
     p.obs_xy[rng.choice(p.n_obs, 200, replace=False)] += 300.0           # tracks that must fail the reprojection test
     p.pt[:] = rng.normal(size=p.pt.shape)                                  # incoming value is ignored
     p.pt_const[::97] = 1                                                   # "already estimated": skipped, bit-identical
+    st = _estimate_and_compare(oracle, p, ba, const=slice(None, None, 97))
+    assert (st == 0).sum() > 4000 and (st == 4).sum() >= 100
+
+
+@pytest.mark.parametrize("ba", [True, False])
+def test_estimate_tracks_on_long_tracks(oracle, ba):
+    """Tracks of 33..256 observations (helpers.long_track_scene): k_estimate_tracks walks each one over the warp slices of a
+    long tile."""
+    p = long_track_scene(seed=33, filler=40, noise_px=0.5, perturb=0.0)
+    rng = np.random.default_rng(2)
+    for q in rng.choice(p.n_pt, 8, replace=False):
+        p.obs_xy[np.nonzero(p.obs_pt == q)[0][:3]] += 300.0              # tracks that must fail the reprojection test
+    p.pt[:] = rng.normal(size=p.pt.shape)
+    p.pt_const[::7] = 1
+    st = _estimate_and_compare(oracle, p, ba, const=slice(None, None, 7))
+    assert (st == 0).sum() >= 40 and (st == 4).sum() >= 5
+
+
+def _estimate_and_compare(oracle, p, ba, const):
     before = p.pt.copy()
     q = p.copy()
     st_o, counts_o = oracle.estimate_tracks(q, oracle.default_options(**KW), bundle_adjustment=ba)
@@ -33,16 +52,28 @@ def test_estimate_tracks_matches_oracle(oracle, model, ba):
     eng.download(p)
     eng.close()
     assert np.array_equal(st, st_o) and np.array_equal(counts, counts_o)
-    assert (st[::97] == 255).all() and np.array_equal(p.pt[::97], before[::97])
+    assert (st[const] == 255).all() and np.array_equal(p.pt[const], before[const])
     ok = st == 0
-    assert ok.sum() > 4000 and (st == 4).sum() >= 100
     tol = 1e-6 if ba else 1e-10
     assert np.abs(euclid(p.pt[ok]) - euclid(q.pt[ok])).max() <= tol * np.abs(euclid(q.pt[ok])).max()
+    return st
 
 
 def test_adjust_tracks_matches_oracle(oracle):
     p = synthetic.make_scene(n_cam=40, n_pt=3000, obs_per_pt=6, seed=19)   # perturbed points, cameras held where they are
     p.pt_const[::50] = 1
+    _adjust_and_compare(oracle, p, const=slice(None, None, 50))
+
+
+def test_adjust_tracks_on_long_tracks(oracle):
+    """BundleAdjustTrack over tracks of 33..256 observations (helpers.long_track_scene), with outliers under HUBER."""
+    p = long_track_scene(seed=19, filler=40)
+    p.pt_const[::9] = 1
+    p.obs_xy[::23] += 30.0
+    _adjust_and_compare(oracle, p, const=slice(None, None, 9))
+
+
+def _adjust_and_compare(oracle, p, const):
     q = p.copy()
     opts = dict(KW, loss_function_type=_abi.LOSS_HUBER, robust_loss_width=3.0)
     st_o, ic_o, fc_o, failed_o = oracle.adjust_tracks(q, oracle.default_options(**opts))
@@ -51,7 +82,7 @@ def test_adjust_tracks_matches_oracle(oracle):
     st, ic, fc, failed = eng.adjust_tracks(engine.default_options(**opts))
     eng.download(p)
     eng.close()
-    assert np.array_equal(st == 255, st_o == 255) and (st[::50] == 255).all()
+    assert np.array_equal(st == 255, st_o == 255) and (st[const] == 255).all()
     live = st != 255
     assert np.allclose(ic[live], ic_o[live], rtol=1e-11)
     # a track that has not converged after max_num_iterations (one of 2940 in the oracle run) sits in a flat valley where

@@ -148,7 +148,7 @@ struct HostPack {  // lives in the engine context: the vectors keep their capaci
   std::vector<int> cam_hist;       // per-thread camera histograms of phase A
   std::vector<int64_t> cursor;     // per-point write cursors of phase C
   std::vector<int64_t> off, order;
-  std::vector<uint8_t> pt_nruns;
+  std::vector<uint16_t> pt_nruns;  // (point, group) runs per point: up to the track length, 256
   // scattered input (observations not grouped by point, e.g. the adapter's per-view flattening): two-level counting sort
   std::vector<int64_t> tmp_idx;    // observation indices grouped by point bucket (stable)
   std::vector<int> tmp_q, tmp_cam; // their point / camera
@@ -398,7 +398,7 @@ inline void pack_count_and_sort(const tba_problem* p, int T, HostPack* H) {
       }
       int runs = 1;
       for (int j = 1; j < n; ++j) runs += (key[j] >> 32) != (key[j - 1] >> 32);
-      H->pt_nruns[q] = (uint8_t)std::min(runs, 255);
+      H->pt_nruns[q] = (uint16_t)runs;
     }
   });
   lap("C per-point sort");
