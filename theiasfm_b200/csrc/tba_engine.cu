@@ -557,7 +557,7 @@ const int* st_done(const PcgState* st) { return reinterpret_cast<const int*>(rei
 // The fused path is available when the whole problem runs through the streaming kernel (no long tiles).
 bool p2p_matvec_possible(const tba_context* c) { return c->p2p_ok && c->p2p_use; }
 
-// defer_fold: the caller folds the shared-intrinsics replica rows itself (k_pcg_a / k_pcg_reset_bz; one GPU only).
+// defer_fold: the caller folds the shared-intrinsics replica rows itself (phase A or RB of k_pcg_fused; one GPU only).
 // pp (world > 1): the matvec kernel itself pushes the partial sums to the peers; no fold launch, no NCCL call.
 int launch_matvec(tba_context* c, const int* done, bool defer_fold = false, const P2pDev& pp = P2pDev()) {
   DevProblem& P = c->P;
@@ -572,15 +572,44 @@ int launch_matvec(tba_context* c, const int* done, bool defer_fold = false, cons
   return allreduce_sum(c, c->y.p, P.ncs);
 }
 
+// The vectors of the CG loop.  One GPU and one shared intrinsics group: phases A and RB fold the matvec's replica rows themselves
+// (no k_fold launch).  Several GPUs with peer memory: the matvec pushes its partial sums to the peers, A and RB sum the inbox.
+PcgVectors pcg_vectors(tba_context* c) {
+  const DevProblem& P = c->P;
+  PcgVectors V;
+  V.sm = c->sm.p; V.D2 = c->D2.p; V.b = c->b.p; V.Minv_c = c->Minv_c.p; V.Minv_i = c->Minv_i.p;
+  V.p = c->p.p; V.q = c->z.p; V.x = c->x.p; V.r = c->r.p; V.z = c->z2.p; V.xs = c->xs.p; V.y = c->y.p;
+  V.part_rho = c->part.p; V.part_pq = c->part.p + VB; V.part_Q = c->part.p + 2 * VB;
+  V.fold_rep = c->world == 1 && P.single_group && P.n_tiles > 0 ? c->rep.p : nullptr;
+  V.zero_ctr = p2p_matvec_possible(c) ? c->p2p_ctr : nullptr;
+  V.bar = c->pcg_bar.p;
+  V.identity_precond = c->opt.preconditioner_type == TBA_PRECOND_IDENTITY;
+  return V;
+}
+
+// One CG step: the phases `mask` (PCG_*) on the state c->st[cur], which moves to the other copy.  On the GPU one k_pcg_fused launch;
+// the emulation build launches the same kernel once per phase.
+int launch_pcg(tba_context* c, const PcgVectors& V, int& cur, int mask, int first, const P2pDev& pp) {
+  PcgState* st = c->st.p;
+#ifdef TBA_EMULATE
+  for (int run = PCG_A; run <= PCG_C; run <<= 1) {
+    if (!(mask & run)) continue;
+    LAUNCH(c, k_pcg_fused, VB, VT, 0, c->P, st + cur, st + (cur ^ 1), V, mask, run, first, pp);
+    cur ^= 1;
+  }
+#else
+  LAUNCH(c, k_pcg_fused, VB, VT, 0, c->P, st + cur, st + (cur ^ 1), V, mask, mask, first, pp);
+  cur ^= 1;
+#endif
+  return TBA_OK;
+}
+
 // ConjugateGradientsSolver::Solve on the reduced system; control flow on the device (PcgState),
 // the host enqueues iterations in batches and polls the done flag.
 // system_ok != nullptr: also fetch stage_prepare's deferred flag (false: the linear system was not usable, the result is void).
 int stage_pcg(tba_context* c, int* iters, int* status, bool* system_ok = nullptr) {
   DevProblem& P = c->P;
   const tba_options& o = c->opt;
-  double* part_rho = c->part.p;
-  double* part_pq = c->part.p + VB;
-  double* part_Q = c->part.p + 2 * VB;
   PcgState* st = c->st.p;
   static const bool trace = getenv("TBA_TRACE_LM") != nullptr;
   cudaEvent_t tev[2] = {nullptr, nullptr};
@@ -593,72 +622,35 @@ int stage_pcg(tba_context* c, int* iters, int* status, bool* system_ok = nullptr
     if (system_ok) { double f; const int rc = read_scal(c, c->flag.p, 1, &f); if (rc) return rc; *system_ok = f == 0.0; }
     return TBA_OK;
   }
-  const int ident = o.preconditioner_type == TBA_PRECOND_IDENTITY;
+  const PcgVectors V = pcg_vectors(c);
+  const bool p2p = p2p_matvec_possible(c);
   int cur = 0;  // index of the valid state
   int it = 0;
-  // Three vector kernels per iteration (k_pcg_c, k_pcg_a, k_pcg_b; tba_kernels.cuh) around the matvec.  One GPU and one shared
-  // intrinsics group: k_pcg_a folds the matvec's replica rows itself (no k_fold launch).  The host enqueues the number of
-  // iterations the previous solve needed (+2) before it looks at the device-side state; surplus iterations early-exit.
-  const bool fold_in_a = c->world == 1 && P.single_group && P.n_tiles > 0;
-  double* fold_rep = fold_in_a ? c->rep.p : nullptr;
-  const bool p2p = p2p_matvec_possible(c);  // multi-GPU: the matvec pushes its partial sums to the peers, k_pcg_a sums the inbox
-  int* zero_ctr = p2p ? c->p2p_ctr : nullptr;
-  // On the GPU: ONE vector kernel per CG iteration -- phases A and B of iteration k and phase C of iteration k + 1 in k_pcg_fused,
-  // grid barriers in between -- i.e. two launches per iteration with the matvec.  The SIMT emulation build runs the CTAs of a
-  // launch one after the other and so cannot run a grid barrier: it launches the three kernels (the same device functions).
-#ifdef TBA_EMULATE
-  constexpr bool fused = false;
-#else
-  constexpr bool fused = true;
-#endif
-  PcgVectors V;
-  V.sm = c->sm.p; V.D2 = c->D2.p; V.b = c->b.p; V.Minv_c = c->Minv_c.p; V.Minv_i = c->Minv_i.p;
-  V.p = c->p.p; V.q = c->z.p; V.x = c->x.p; V.r = c->r.p; V.z = c->z2.p; V.xs = c->xs.p; V.y = c->y.p;
-  V.part_pq = part_pq; V.part_Q = part_Q; V.part_rho = part_rho; V.fold_rep = fold_rep; V.zero_ctr = zero_ctr; V.bar = c->pcg_bar.p;
-  V.identity_precond = ident;
-  if (fused) {  // z = Minv r, rho (phase B, first) and phase C of iteration 1
-    LAUNCH(c, k_pcg_fused, VB, VT, 0, P, st + cur, st + (cur ^ 1), V, 2 | 4, 1, p2p_none());
-    cur ^= 1;
-  } else {
-    LAUNCH(c, k_pcg_b, VB, VT, 0, P, st + cur, st + (cur ^ 1), part_pq, c->p.p, c->z.p, c->b.p, c->x.p, c->r.p, c->z2.p, c->Minv_c.p, c->Minv_i.p,
-           part_Q, part_rho, ident, 1, nullptr);
-    cur ^= 1;
-  }
-  bool c_pending = !fused;  // phase C of the coming iteration still to be launched (split mode: always; fused: after a residual reset)
+  // Two launches per CG iteration: the matvec and k_pcg_fused (tba_kernels.cuh).  The host enqueues the number of iterations the
+  // previous solve needed (+2) before it looks at the device-side state; surplus iterations early-exit.
+  int rc = launch_pcg(c, V, cur, PCG_B | PCG_C, 1, p2p_none());  // z = Minv r, rho, and phase C of iteration 1
+  if (rc) return rc;
   int batch = std::max(4, std::min(c->last_cg_iters + 2, 64));
   for (;;) {
     for (int k = 0; k < batch; ++k) {
       ++it;
-      if (c_pending) {
-        LAUNCH(c, k_pcg_c, VB, VT, 0, P.ncs, st + cur, st + (cur ^ 1), part_Q, part_rho, c->z2.p, c->sm.p, c->p.p, c->xs.p, c->y.p, nullptr, zero_ctr);
-        cur ^= 1;
-      }
       // every kernel of an iteration (matvec included) early-exits through the device-side state
       const P2pDev pp = p2p ? p2p_next(c) : p2p_none();
-      int rc = launch_matvec(c, st_done(st + cur), fold_in_a, pp);
+      rc = launch_matvec(c, st_done(st + cur), V.fold_rep != nullptr, pp);
       if (rc) return rc;
-      const bool reset_now = o.cg_residual_reset_period > 0 && it % o.cg_residual_reset_period == 0;
-      if (fused) {
-        LAUNCH(c, k_pcg_fused, VB, VT, 0, P, st + cur, st + (cur ^ 1), V, reset_now ? (1 | 2) : (1 | 2 | 4), 0, pp);
-        cur ^= 1;
-        c_pending = reset_now;
-      } else {
-        LAUNCH(c, k_pcg_a, VB, VT, 0, P.ncs, P.ne, st + cur, c->y.p, c->sm.p, c->D2.p, c->p.p, c->z.p, part_pq, fold_rep, pp);
-        LAUNCH(c, k_pcg_b, VB, VT, 0, P, st + cur, st + (cur ^ 1), part_pq, c->p.p, c->z.p, c->b.p, c->x.p, c->r.p, c->z2.p, c->Minv_c.p, c->Minv_i.p,
-               part_Q, part_rho, ident, 0, fold_rep);
-        cur ^= 1;
-      }
-      if (reset_now) {
-        LAUNCH(c, k_pcg_reset_a, VB, VT, 0, P.ncs, st + cur, c->x.p, c->sm.p, c->xs.p, c->y.p, zero_ctr);
-        const P2pDev pr = p2p ? p2p_next(c) : p2p_none();
-        rc = launch_matvec(c, st_done(st + cur), fold_in_a, pr);
+      if (o.cg_residual_reset_period > 0 && it % o.cg_residual_reset_period == 0) {
+        rc = launch_pcg(c, V, cur, PCG_A | PCG_B | PCG_RA, 0, pp);
         if (rc) return rc;
-        LAUNCH(c, k_pcg_reset_bz, VB, VT, 0, P, st + cur, c->y.p, c->sm.p, c->D2.p, c->x.p, c->b.p, c->r.p, c->z2.p, c->Minv_c.p, c->Minv_i.p,
-               part_Q, part_rho, ident, fold_rep, pr);
-        if (fold_in_a) LAUNCH(c, k_zero_rep_cols, 4, 256, 0, c->rep.p);
+        const P2pDev pr = p2p ? p2p_next(c) : p2p_none();
+        rc = launch_matvec(c, st_done(st + cur), V.fold_rep != nullptr, pr);
+        if (rc) return rc;
+        rc = launch_pcg(c, V, cur, PCG_RB | PCG_C, 0, pr);
+      } else {
+        rc = launch_pcg(c, V, cur, PCG_A | PCG_B | PCG_C, 0, pp);
       }
+      if (rc) return rc;
     }
-    LAUNCH(c, k_pcg_finalize, 1, 32, 0, st + cur, st + (cur ^ 1), part_Q, c->done_flag.p);
+    LAUNCH(c, k_pcg_finalize, 1, 32, 0, st + cur, st + (cur ^ 1), V.part_Q, c->done_flag.p);
     cur ^= 1;
     CUDA_OK(c, cudaMemcpyAsync(c->h_st, st + cur, sizeof(PcgState), cudaMemcpyDeviceToHost, c->stream));
     if (system_ok) CUDA_OK(c, cudaMemcpyAsync(c->h_scal, c->flag.p, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
@@ -2116,7 +2108,11 @@ int tba_debug_schur_matvec(tba_context* c, const double* x_cam, const double* x_
   int rc = launch_matvec(c, c->done_flag.p);
   if (rc) return rc;
   LAUNCH(c, k_set_flag, 1, 1, 0, const_cast<int*>(st_done(c->st.p)), 0);
-  LAUNCH(c, k_pcg_v3, VB, VT, 0, P.ncs, c->st.p, c->y.p, c->sm.p, c->D2.p, c->p.p, c->z.p, c->part.p + VB);
+  PcgVectors V = pcg_vectors(c);  // phase A on the folded y: no fold of its own, no peer sums
+  V.fold_rep = nullptr;
+  int cur = 0;
+  rc = launch_pcg(c, V, cur, PCG_A, 0, p2p_none());
+  if (rc) return rc;
   CUDA_OK(c, cudaMemcpyAsync(y_cam, c->z.p, (size_t)P.ne * 8, cudaMemcpyDeviceToHost, c->stream));
   CUDA_OK(c, cudaMemcpyAsync(y_intr, c->z.p + P.ne, (size_t)P.n_group * 10 * 8, cudaMemcpyDeviceToHost, c->stream));
   CUDA_OK(c, cudaStreamSynchronize(c->stream));

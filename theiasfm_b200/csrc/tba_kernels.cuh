@@ -819,7 +819,7 @@ __global__ void __launch_bounds__(TILE, (14 + 2 * popcount10(IMASK)) <= 20 ? 4 :
 // Every rank owns an "inbox" [2][world][cap] in its own HBM that all peers can write (CUDA IPC / peer access).  After a grid
 // barrier inside k_schur_stream<., 0> (its persistent CTAs are co-resident) every CTA STORES its slice of the rank's complete
 // partial y into slot `rank` of every peer's inbox (buffer seq & 1) -- 16-byte stores over NVLink from all SMs, no separate
-// collective launch -- and the CTA that finishes last releases flags[rank] = seq on every peer.  The consumer (k_pcg_a / k_pcg_reset_bz) acquires the `world` flags of its own
+// collective launch -- and the CTA that finishes last releases flags[rank] = seq on every peer.  The consumer (phase A or RB of k_pcg_fused) acquires the `world` flags of its own
 // inbox and sums the slots in rank order: the same bits on every rank (the replicated PCG state stays in lockstep) and
 // run-to-run reproducible for a given world size.  Two buffers suffice: a rank can be at most one exchange ahead of a peer,
 // because exchange k+1 needs the sums of exchange k, to which every peer contributed after it consumed exchange k-1.
@@ -829,7 +829,7 @@ struct P2pDev {
   size_t cap = 0;                        // doubles per slot
   double* const* inbox = nullptr;        // [world] base pointers of the ranks' inboxes (inbox[rank] is the local one)
   unsigned long long* const* flags = nullptr;  // [world] base pointers of the ranks' flag arrays ([world] each)
-  int* ctr = nullptr;                    // local counters [2]: CTAs at the grid barrier / CTAs done pushing (zeroed before every matvec by k_pcg_c / k_pcg_reset_a)
+  int* ctr = nullptr;                    // local counters [2]: CTAs at the grid barrier / CTAs done pushing (zeroed before every matvec by phase C or RA of k_pcg_fused)
 };
 #ifdef TBA_EMULATE
 __device__ __forceinline__ void st_release_sys(unsigned long long* p, unsigned long long v) { *p = v; }
@@ -1892,7 +1892,7 @@ __global__ void k_cs_diag(int ncs, const double* __restrict__ cn, const double* 
     D2[i] = sm[i] != 0.0 ? fmin(fmax(sm[i] * sm[i] * cn[i], lo), hi) / radius : 0.0;
 }
 
-// PCG state (ping-pong between kernels; see DESIGN.md section 5.4).
+// PCG state: two copies, every kernel of a CG solve that updates it (k_pcg_fused, k_pcg_finalize) reads one and writes the other.
 struct PcgState {
   double rho, last_rho, beta, alpha, pq, Q0, Q1, norm_b2;
   int iters;        // current (1-based) iteration
@@ -1943,30 +1943,17 @@ __global__ void k_pcg_init_state(PcgState* st, const double* __restrict__ part, 
   *st = s;
 }
 
-// q = sm .* y + D2 .* p; partial pq = p.q  (kept for tba_debug_schur_matvec)
-__global__ void __launch_bounds__(VT) k_pcg_v3(int ncs, const PcgState* __restrict__ in, const double* __restrict__ y,
-                                               const double* __restrict__ sm, const double* __restrict__ D2,
-                                               const double* __restrict__ p, double* __restrict__ q,
-                                               double* __restrict__ part_pq) {
-  __shared__ double s_red[32];
-  if (in->done) return;
-  double acc = 0.0;
-  for (int i = blockIdx.x * VT + threadIdx.x; i < ncs; i += VB * VT) {
-    const double qv = sm[i] * y[i] + D2[i] * p[i];
-    q[i] = qv;
-    acc += p[i] * qv;
-  }
-  const double s = block_sum(acc, s_red);
-  if (threadIdx.x == 0) part_pq[blockIdx.x] = s;
-}
-
-// ---- round 2: three vector kernels per CG iteration instead of four (plus the separate fold) -------------------------------
-//   C: [Q-test of the previous iteration]; rho, beta; p = z + beta p; xs = sm .* p; y = 0        (k_pcg_c)
-//      matvec
-//   A: [fold of the shared-intrinsics replica rows into y]; q = sm .* y + D2 .* p; partial p.q   (k_pcg_a)
-//   B: alpha = rho / pq; x += alpha p; r -= alpha q; partial x.(b + r); z = Minv r; partial r.z  (k_pcg_b, per parameter block)
-// The same operations in the same order as the round-1 sequence k_pcg_v1 .. v4; the partial sums of x.(b + r) are grouped per
-// parameter block now (they were grouped per element stride), i.e. equal up to fp64 summation order.
+// ---- the vector phases of the CG iterations, around the matvec:
+//   C:  [Q-test of the previous iteration]; rho, beta; p = z + beta p; xs = sm .* p; y = 0
+//       matvec
+//   A:  [fold of the shared-intrinsics replica rows into y]; q = sm .* y + D2 .* p; partial p.q
+//   B:  alpha = rho / pq; x += alpha p; r -= alpha q; partial x.(b + r); z = Minv r; partial r.z  (per parameter block)
+// and every cg_residual_reset_period iterations the true residual instead of r -= alpha q, from one more matvec:
+//   RA: xs = sm .* x; y = 0
+//       matvec
+//   RB: [fold]; r = b - (sm .* y + D2 .* x); partial x.(b + r); z = Minv r; partial r.z    (per parameter block)
+// The operations of ConjugateGradientsSolver in its order; the partial sums of x.(b + r) are grouped per parameter block, i.e.
+// equal up to fp64 summation order.
 
 // z = Minv r for one parameter block (camera: 6, intrinsics group: 10); returns r.z
 __device__ __forceinline__ double pcg_precondition_block(const DevProblem& P, int blk, const double* __restrict__ Minv_c,
@@ -2029,11 +2016,36 @@ __device__ __forceinline__ void pcg_q_test(PcgState& st, const double* __restric
   }
 }
 
-// The three phases as device functions on a PcgState held in registers (every CTA computes the same state from the same partial
-// sums): the kernels k_pcg_c / k_pcg_a / k_pcg_b wrap one phase each, k_pcg_fused runs them back to back with grid barriers.
+// The phases as device functions on a PcgState held in registers (every CTA computes the same state from the same partial sums).
+
+// The y of a matvec as phases A and RB read it.  Several GPUs: the peers' partial sums in the local inbox.  One GPU and one shared
+// intrinsics group (fold_rep != nullptr): the replica rows of the matvec folded into y[ne ..] in the fixed row order of k_fold, by
+// every CTA (they all need the value); the phase behind the next grid barrier re-zeroes the replicas (pcg_zero_rep).
+__device__ __forceinline__ void pcg_take_y(int ne, const double* __restrict__ y, const double* __restrict__ fold_rep,
+                                           const P2pDev& pp, double* s_fold) {
+  if (pp.world > 1) p2p_wait(pp);  // the matvec of every rank has pushed its partial sums into the local inbox
+  if (fold_rep != nullptr) {
+    if (threadIdx.x < 10) {
+      double v = y[ne + threadIdx.x];
+      for (int r = 0; r < NREP; ++r) v += fold_rep[(size_t)r * REPW + threadIdx.x];
+      s_fold[threadIdx.x] = v;
+    }
+    __syncthreads();
+  }
+}
+__device__ __forceinline__ double pcg_y(int i, int ne, const double* __restrict__ y, const double* __restrict__ fold_rep,
+                                        const P2pDev& pp, const double* s_fold) {
+  return pp.world > 1 ? p2p_sum(pp, i) : ((fold_rep != nullptr && i >= ne && i < ne + 10) ? s_fold[i - ne] : y[i]);
+}
+__device__ __forceinline__ void pcg_zero_rep(double* __restrict__ rep) {  // the 10 replica columns a fold has read
+  for (int i = blockIdx.x * VT + threadIdx.x; i < NREP * 10; i += VB * VT) rep[(size_t)(i / 10) * REPW + (i % 10)] = 0.0;
+}
+
 __device__ __forceinline__ void pcg_phase_c(int ncs, PcgState& st, const double* __restrict__ part_Q, const double* __restrict__ part_rho,
                                             const double* __restrict__ z, const double* __restrict__ sm, double* __restrict__ p,
-                                            double* __restrict__ xs, double* __restrict__ y, int* __restrict__ zero_ctr, double* s_red) {
+                                            double* __restrict__ xs, double* __restrict__ y, int* __restrict__ zero_ctr,
+                                            double* __restrict__ zero_rep, double* s_red) {
+  if (zero_rep != nullptr) pcg_zero_rep(zero_rep);  // the replica columns folded by phase RB
   if (zero_ctr != nullptr && blockIdx.x == 0 && threadIdx.x == 0) { zero_ctr[0] = 0; zero_ctr[1] = 0; }  // barrier / completion counters of the next matvec
   pcg_q_test(st, part_Q, s_red);
   if (!st.done) {
@@ -2056,35 +2068,16 @@ __device__ __forceinline__ void pcg_phase_c(int ncs, PcgState& st, const double*
     y[i] = 0.0;
   }
 }
-__global__ void __launch_bounds__(VT) k_pcg_c(int ncs, const PcgState* __restrict__ in, PcgState* __restrict__ out,
-                                              const double* __restrict__ part_Q, const double* __restrict__ part_rho,
-                                              const double* __restrict__ z, const double* __restrict__ sm, double* __restrict__ p,
-                                              double* __restrict__ xs, double* __restrict__ y, int* __restrict__ done_flag, int* __restrict__ zero_ctr) {
-  __shared__ double s_red[32];
-  PcgState st = *in;
-  pcg_phase_c(ncs, st, part_Q, part_rho, z, sm, p, xs, y, zero_ctr, s_red);
-  if (blockIdx.x == 0 && threadIdx.x == 0) { *out = st; if (done_flag) *done_flag = st.done; }
-}
 
-// fold_rep != nullptr (one GPU, one shared intrinsics group): the replica rows of the matvec are folded into y[ne ..] here,
-// in the fixed row order of k_fold, by every CTA (they all need the value) -- CTA 0 stores it and re-zeroes the replicas.
-__device__ __forceinline__ void pcg_phase_a(int ncs, int ne, double* __restrict__ y, const double* __restrict__ sm,
+__device__ __forceinline__ void pcg_phase_a(int ncs, int ne, const double* __restrict__ y, const double* __restrict__ sm,
                                             const double* __restrict__ D2, const double* __restrict__ p, double* __restrict__ q,
                                             double* __restrict__ part_pq, const double* __restrict__ fold_rep, const P2pDev& pp,
                                             double* s_red, double* s_fold) {
-  if (pp.world > 1) p2p_wait(pp);  // the matvec of every rank has pushed its partial sums into the local inbox
-  if (fold_rep != nullptr) {
-    if (threadIdx.x < 10) {
-      double v = y[ne + threadIdx.x];
-      for (int r = 0; r < NREP; ++r) v += fold_rep[(size_t)r * REPW + threadIdx.x];
-      s_fold[threadIdx.x] = v;
-    }
-    __syncthreads();
-  }
+  pcg_take_y(ne, y, fold_rep, pp, s_fold);
   double acc = 0.0;
 #pragma unroll 4
   for (int i = blockIdx.x * VT + threadIdx.x; i < ncs; i += VB * VT) {
-    const double yv = pp.world > 1 ? p2p_sum(pp, i) : ((fold_rep != nullptr && i >= ne && i < ne + 10) ? s_fold[i - ne] : y[i]);
+    const double yv = pcg_y(i, ne, y, fold_rep, pp, s_fold);
     const double qv = sm[i] * yv + D2[i] * p[i];
     q[i] = qv;
     acc += p[i] * qv;
@@ -2092,16 +2085,6 @@ __device__ __forceinline__ void pcg_phase_a(int ncs, int ne, double* __restrict_
   const double s = block_sum(acc, s_red);
   if (threadIdx.x == 0) part_pq[blockIdx.x] = s;
 }
-__global__ void __launch_bounds__(VT) k_pcg_a(int ncs, int ne, const PcgState* __restrict__ in, double* __restrict__ y,
-                                              const double* __restrict__ sm, const double* __restrict__ D2,
-                                              const double* __restrict__ p, double* __restrict__ q, double* __restrict__ part_pq,
-                                              const double* __restrict__ fold_rep, P2pDev pp) {
-  __shared__ double s_red[32];
-  __shared__ double s_fold[10];
-  if (in->done) return;
-  pcg_phase_a(ncs, ne, y, sm, D2, p, q, part_pq, fold_rep, pp, s_red, s_fold);
-}
-// (the replicas are re-zeroed by the kernel that runs after every CTA of k_pcg_a has read them: k_pcg_b)
 
 __device__ __forceinline__ void pcg_phase_b(const DevProblem& P, PcgState& st, const double* __restrict__ part_pq,
                                             const double* __restrict__ p, const double* __restrict__ q, const double* __restrict__ b,
@@ -2119,9 +2102,7 @@ __device__ __forceinline__ void pcg_phase_b(const DevProblem& P, PcgState& st, c
       else st.pending_q = 1;
     }
   }
-  if (zero_rep != nullptr && !first) {  // the replica columns folded by phase A
-    for (int i = blockIdx.x * VT + threadIdx.x; i < NREP * 10; i += VB * VT) zero_rep[(size_t)(i / 10) * REPW + (i % 10)] = 0.0;
-  }
+  if (zero_rep != nullptr) pcg_zero_rep(zero_rep);  // the replica columns folded by phase A
   if (st.done) return;
   double accQ = 0.0, accR = 0.0;
   const int nblk = P.n_cam + P.n_group;
@@ -2142,23 +2123,43 @@ __device__ __forceinline__ void pcg_phase_b(const DevProblem& P, PcgState& st, c
   const double sR = block_sum(accR, s_red);
   if (threadIdx.x == 0) { if (!first) part_Q[blockIdx.x] = sQ; part_rho[blockIdx.x] = sR; }
 }
-__global__ void __launch_bounds__(VT) k_pcg_b(DevProblem P, const PcgState* __restrict__ in, PcgState* __restrict__ out,
-                                              const double* __restrict__ part_pq, const double* __restrict__ p,
-                                              const double* __restrict__ q, const double* __restrict__ b, double* __restrict__ x,
-                                              double* __restrict__ r, double* __restrict__ z, const double* __restrict__ Minv_c,
-                                              const double* __restrict__ Minv_i, double* __restrict__ part_Q,
-                                              double* __restrict__ part_rho, int identity_precond, int first, double* __restrict__ zero_rep) {
-  __shared__ double s_red[32];
-  PcgState st = *in;
-  pcg_phase_b(P, st, part_pq, p, q, b, x, r, z, Minv_c, Minv_i, part_Q, part_rho, identity_precond, first, zero_rep, s_red);
-  if (blockIdx.x == 0 && threadIdx.x == 0) *out = st;
+
+__device__ __forceinline__ void pcg_phase_ra(int ncs, const double* __restrict__ x, const double* __restrict__ sm,
+                                             double* __restrict__ xs, double* __restrict__ y, int* __restrict__ zero_ctr) {
+  if (zero_ctr != nullptr && blockIdx.x == 0 && threadIdx.x == 0) { zero_ctr[0] = 0; zero_ctr[1] = 0; }  // counters of the reset matvec
+  for (int i = blockIdx.x * VT + threadIdx.x; i < ncs; i += VB * VT) { xs[i] = sm[i] * x[i]; y[i] = 0.0; }
 }
 
-// ---- the three phases in ONE launch (one GPU kernel per CG iteration next to the matvec): A -> grid barrier -> B -> grid barrier
-// -> C of the NEXT iteration.  VB CTAs of VT threads are co-resident on any device this engine runs on (the previous kernel of the
-// stream has finished).  Sense-reversal barrier on bar[0] (arrivals) / bar[1] (generation), both zero before the first use; the
-// partial sums written before a barrier are read behind it (fence by the arriving thread, cumulative through the block barrier).
-// phase_mask: bit 0 = A, bit 1 = B, bit 2 = C (an iteration followed by a residual reset runs A|B only, the reset kernels, then C).
+// the residual reset with the preconditioner applied to the fresh residual
+__device__ __forceinline__ void pcg_phase_rb(const DevProblem& P, const double* __restrict__ y, const double* __restrict__ sm,
+                                             const double* __restrict__ D2, const double* __restrict__ x, const double* __restrict__ b,
+                                             double* __restrict__ r, double* __restrict__ z, const double* __restrict__ Minv_c,
+                                             const double* __restrict__ Minv_i, double* __restrict__ part_Q, double* __restrict__ part_rho,
+                                             int identity_precond, const double* __restrict__ fold_rep, const P2pDev& pp,
+                                             double* s_red, double* s_fold) {
+  pcg_take_y(P.ne, y, fold_rep, pp, s_fold);
+  double accQ = 0.0, accR = 0.0;
+  const int nblk = P.n_cam + P.n_group;
+  for (int blk = blockIdx.x * VT + threadIdx.x; blk < nblk; blk += VB * VT) {
+    const int i0 = blk < P.n_cam ? blk * 6 : P.ne + (blk - P.n_cam) * 10, n = blk < P.n_cam ? 6 : 10;
+    for (int a = 0; a < n; ++a) {
+      const int i = i0 + a;
+      const double yv = pcg_y(i, P.ne, y, fold_rep, pp, s_fold);
+      const double rv = b[i] - (sm[i] * yv + D2[i] * x[i]);
+      r[i] = rv;
+      accQ += x[i] * (b[i] + rv);
+    }
+    accR += pcg_precondition_block(P, blk, Minv_c, Minv_i, r, z, identity_precond);
+  }
+  const double sQ = block_sum(accQ, s_red);
+  const double sR = block_sum(accR, s_red);
+  if (threadIdx.x == 0) { part_Q[blockIdx.x] = sQ; part_rho[blockIdx.x] = sR; }
+}
+
+// ---- the phases of one CG step in ONE launch, a grid barrier between two phases (a phase reads what other CTAs wrote before it).
+// VB CTAs of VT threads are co-resident on any device this engine runs on (the previous kernel of the stream has finished).
+// Sense-reversal barrier on bar[0] (arrivals) / bar[1] (generation), both zero before the first use; the partial sums written
+// before a barrier are read behind it (fence by the arriving thread, cumulative through the block barrier).
 __device__ __forceinline__ void pcg_grid_barrier(int* bar) {
   __syncthreads();
   if (threadIdx.x == 0) {
@@ -2184,13 +2185,19 @@ struct PcgVectors {
   const double *sm, *D2, *b, *Minv_c, *Minv_i;
   double *p, *q, *x, *r, *z, *xs, *y;
   double *part_pq, *part_Q, *part_rho;
-  double* fold_rep;  // shared-intrinsics replica rows folded by phase A (one GPU), or nullptr
+  double* fold_rep;  // shared-intrinsics replica rows folded by phases A and RB (one GPU), or nullptr
   int* zero_ctr;     // P2P counters of the next matvec, or nullptr
   int* bar;          // [2] grid barrier
   int identity_precond;
 };
+// Phase bits; the phases of a step run in bit order.  A CG iteration is the matvec and A|B|C (C of the next iteration); an
+// iteration with a residual reset is the matvec, A|B|RA, the reset matvec and RB|C.  The start of a solve is B|C with first = 1.
+enum { PCG_A = 1, PCG_B = 2, PCG_RA = 4, PCG_RB = 8, PCG_C = 16 };
+// mask: the phases of the step; it decides which phase re-zeroes the replica columns of a fold (B after A, C after RB).
+// run: the phases this launch runs -- the whole mask on the GPU, one phase per launch in the emulation build (its CTAs run one
+// after the other and cannot pass a grid barrier).
 __global__ void __launch_bounds__(VT) k_pcg_fused(DevProblem P, const PcgState* __restrict__ in, PcgState* __restrict__ out, PcgVectors V,
-                                                  int phase_mask, int first, P2pDev pp) {
+                                                  int mask, int run, int first, P2pDev pp) {
   __shared__ double s_red[32];
   __shared__ double s_fold[10];
   PcgState st = *in;
@@ -2198,85 +2205,41 @@ __global__ void __launch_bounds__(VT) k_pcg_fused(DevProblem P, const PcgState* 
     if (blockIdx.x == 0 && threadIdx.x == 0) *out = st;
     return;
   }
-  if (phase_mask & 1) {
+  bool after = false;  // a phase of this launch has run: the next one waits at a grid barrier
+  if (run & PCG_A) {
     pcg_phase_a(P.ncs, P.ne, V.y, V.sm, V.D2, V.p, V.q, V.part_pq, V.fold_rep, pp, s_red, s_fold);
-    if (phase_mask & 6) pcg_grid_barrier(V.bar);
+    after = true;
   }
-  if (phase_mask & 2) {
+  if (run & PCG_B) {
+    if (after) pcg_grid_barrier(V.bar);
     pcg_phase_b(P, st, V.part_pq, V.p, V.q, V.b, V.x, V.r, V.z, V.Minv_c, V.Minv_i, V.part_Q, V.part_rho, V.identity_precond, first,
-                (phase_mask & 1) ? V.fold_rep : nullptr, s_red);
-    if (!st.done && (phase_mask & 4)) pcg_grid_barrier(V.bar);
+                (mask & PCG_A) ? V.fold_rep : nullptr, s_red);
+    after = true;
   }
-  if ((phase_mask & 4) && !st.done) pcg_phase_c(P.ncs, st, V.part_Q, V.part_rho, V.z, V.sm, V.p, V.xs, V.y, V.zero_ctr, s_red);
+  if ((run & PCG_RA) && !st.done) {
+    if (after) pcg_grid_barrier(V.bar);
+    pcg_phase_ra(P.ncs, V.x, V.sm, V.xs, V.y, V.zero_ctr);
+    after = true;
+  }
+  if (run & PCG_RB) {
+    if (after) pcg_grid_barrier(V.bar);
+    pcg_phase_rb(P, V.y, V.sm, V.D2, V.x, V.b, V.r, V.z, V.Minv_c, V.Minv_i, V.part_Q, V.part_rho, V.identity_precond, V.fold_rep, pp,
+                 s_red, s_fold);
+    after = true;
+  }
+  if ((run & PCG_C) && !st.done) {
+    if (after) pcg_grid_barrier(V.bar);
+    pcg_phase_c(P.ncs, st, V.part_Q, V.part_rho, V.z, V.sm, V.p, V.xs, V.y, V.zero_ctr, (mask & PCG_RB) ? V.fold_rep : nullptr, s_red);
+  }
   if (blockIdx.x == 0 && threadIdx.x == 0) *out = st;
 }
 
-// Residual reset, second half, with the preconditioner applied to the fresh residual: r = b - (sm.*y + D2.*x); partial x.(b + r);
-// z = Minv r; partial r.z (per parameter block)
-__global__ void __launch_bounds__(VT) k_pcg_reset_bz(DevProblem P, const PcgState* __restrict__ in, double* __restrict__ y,
-                                                     const double* __restrict__ sm, const double* __restrict__ D2,
-                                                     const double* __restrict__ x, const double* __restrict__ b, double* __restrict__ r,
-                                                     double* __restrict__ z, const double* __restrict__ Minv_c,
-                                                     const double* __restrict__ Minv_i, double* __restrict__ part_Q,
-                                                     double* __restrict__ part_rho, int identity_precond, const double* __restrict__ fold_rep, P2pDev pp) {
-  __shared__ double s_red[32];
-  __shared__ double s_fold[10];
-  if (in->done) return;
-  if (pp.world > 1) p2p_wait(pp);
-  if (fold_rep != nullptr) {
-    if (threadIdx.x < 10) {
-      double v = y[P.ne + threadIdx.x];
-      for (int rr = 0; rr < NREP; ++rr) v += fold_rep[(size_t)rr * REPW + threadIdx.x];
-      s_fold[threadIdx.x] = v;
-    }
-    __syncthreads();
-  }
-  double accQ = 0.0, accR = 0.0;
-  const int nblk = P.n_cam + P.n_group;
-  for (int blk = blockIdx.x * VT + threadIdx.x; blk < nblk; blk += VB * VT) {
-    const int i0 = blk < P.n_cam ? blk * 6 : P.ne + (blk - P.n_cam) * 10, n = blk < P.n_cam ? 6 : 10;
-    for (int a = 0; a < n; ++a) {
-      const int i = i0 + a;
-      const double yv = pp.world > 1 ? p2p_sum(pp, i) : ((fold_rep != nullptr && i >= P.ne && i < P.ne + 10) ? s_fold[i - P.ne] : y[i]);
-      const double rv = b[i] - (sm[i] * yv + D2[i] * x[i]);
-      r[i] = rv;
-      accQ += x[i] * (b[i] + rv);
-    }
-    accR += pcg_precondition_block(P, blk, Minv_c, Minv_i, r, z, identity_precond);
-  }
-  const double sQ = block_sum(accQ, s_red);
-  const double sR = block_sum(accR, s_red);
-  if (threadIdx.x == 0) { part_Q[blockIdx.x] = sQ; part_rho[blockIdx.x] = sR; }
-}
-__global__ void k_zero_rep_cols(double* __restrict__ rep) {  // re-zero the 10 folded replica columns (after k_pcg_reset_bz)
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < NREP * 10; i += gridDim.x * blockDim.x) rep[(size_t)(i / 10) * REPW + (i % 10)] = 0.0;
-}
-
-// Residual reset (every cg_residual_reset_period iterations): xs = sm .* x, y = 0 ... matvec ... r = b - (sm.*y + D2.*x)
-__global__ void __launch_bounds__(VT) k_pcg_reset_a(int ncs, const PcgState* __restrict__ in, const double* __restrict__ x,
-                                                    const double* __restrict__ sm, double* __restrict__ xs, double* __restrict__ y,
-                                                    int* __restrict__ zero_ctr) {
-  if (zero_ctr != nullptr && blockIdx.x == 0 && threadIdx.x == 0) { zero_ctr[0] = 0; zero_ctr[1] = 0; }
-  if (in->done) return;
-  for (int i = blockIdx.x * VT + threadIdx.x; i < ncs; i += VB * VT) { xs[i] = sm[i] * x[i]; y[i] = 0.0; }
-}
 // Finalise a batch: run the pending Q-test so that `done`/`iters` are current, publish the flag.
 __global__ void k_pcg_finalize(const PcgState* __restrict__ in, PcgState* __restrict__ out, const double* __restrict__ part_Q,
                                int* __restrict__ done_flag) {
   __shared__ double s_red[32];
   PcgState st = *in;
-  if (!st.done && st.pending_q) {
-    const double Q1 = -sum_partials(part_Q, s_red);
-    const double zeta = st.iters * (Q1 - st.Q0) / Q1;
-    st.Q1 = Q1;
-    st.pending_q = 0;
-    if (zeta < st.eta && st.iters >= st.min_iters) { st.done = 1; st.status = 0; }
-    else {
-      st.Q0 = Q1;
-      if (st.iters >= st.max_iters) { st.done = 1; st.status = 1; }
-      else st.iters += 1;
-    }
-  }
+  pcg_q_test(st, part_Q, s_red);
   if (threadIdx.x == 0) { *out = st; *done_flag = st.done; }
 }
 __global__ void k_set_flag(int* f, int v) { *f = v; }
