@@ -184,6 +184,173 @@ __device__ __forceinline__ int run_head_lane(unsigned heads, int lane) { return 
 // Element (row k, lane) of the per-warp slice of a [tile][warp][rows][32] array.
 __device__ __forceinline__ size_t wslice(int tile, int warp, int rows) { return ((size_t)tile * (TILE / 32) + warp) * rows * 32; }
 
+__device__ __forceinline__ void sym4_mul(const double* __restrict__ M, const double t[4], double u[4]) {
+  u[0] = M[0] * t[0] + M[1] * t[1] + M[2] * t[2] + M[3] * t[3];
+  u[1] = M[1] * t[0] + M[4] * t[1] + M[5] * t[2] + M[6] * t[3];
+  u[2] = M[2] * t[0] + M[5] * t[1] + M[7] * t[2] + M[8] * t[3];
+  u[3] = M[3] * t[0] + M[6] * t[1] + M[8] * t[2] + M[9] * t[3];
+}
+
+// ---------------------------------------------------- per-observation algebra of the passes over J
+// One observation's rows of the compact Jacobian: J_p = [J_a | J_h] (point, 2 x 4), J_c = [-h J_a | J_w] (camera, 2 x 6) and
+// J_i (the NI intrinsics columns of IMASK); element k of J_a is row k / 3, column k % 3 (J_w and J_i alike).  The tile kernels
+// and the streaming kernels compute every per-observation term with these helpers, so the two families round alike: a
+// change to an expression here changes both.  A row set is a pointer plus a compile-time element stride: 32 for a warp's
+// shared-memory stage ([row][32 lanes]), 1 for a register array.  SP: stride of J_a and J_h; SC: stride of J_w and J_i.
+
+// w = F x = J_c x_c + J_i x_i
+template <int NI, int SP, int SC>
+__device__ __forceinline__ void obs_apply_F(const double* ja, const double* jw, const double* ji, double h, double2 xa, double2 xb,
+                                            double2 xc, const double* xi, double& w0, double& w1) {
+  w0 = -h * (ja[0] * xa.x + ja[SP] * xa.y + ja[2 * SP] * xb.x) + jw[0] * xb.y + jw[SC] * xc.x + jw[2 * SC] * xc.y;
+  w1 = -h * (ja[3 * SP] * xa.x + ja[4 * SP] * xa.y + ja[5 * SP] * xb.x) + jw[3 * SC] * xb.y + jw[4 * SC] * xc.x + jw[5 * SC] * xc.y;
+#pragma unroll
+  for (int j = 0; j < NI; ++j) { w0 += ji[j * SC] * xi[j]; w1 += ji[(NI + j) * SC] * xi[j]; }
+}
+// t = J_p^T w
+template <int SP>
+__device__ __forceinline__ void obs_JpT(const double* ja, const double* jh, double w0, double w1, double t[4]) {
+  t[0] = ja[0] * w0 + ja[3 * SP] * w1; t[1] = ja[SP] * w0 + ja[4 * SP] * w1; t[2] = ja[2 * SP] * w0 + ja[5 * SP] * w1;
+  t[3] = jh[0] * w0 + jh[SP] * w1;
+}
+// z = w - J_p u
+template <int SP>
+__device__ __forceinline__ void obs_sub_Jp(const double* ja, const double* jh, double w0, double w1, const double u[4], double& z0, double& z1) {
+  z0 = w0 - (ja[0] * u[0] + ja[SP] * u[1] + ja[2 * SP] * u[2] + jh[0] * u[3]);
+  z1 = w1 - (ja[3 * SP] * u[0] + ja[4 * SP] * u[1] + ja[5 * SP] * u[2] + jh[SP] * u[3]);
+}
+// y_c = J_c^T z
+template <int SP, int SC>
+__device__ __forceinline__ void obs_JcT(const double* ja, const double* jw, double h, double z0, double z1, double y[6]) {
+#pragma unroll
+  for (int j = 0; j < 3; ++j) y[j] = -h * (ja[j * SP] * z0 + ja[(3 + j) * SP] * z1);
+#pragma unroll
+  for (int j = 0; j < 3; ++j) y[3 + j] = jw[j * SC] * z0 + jw[(3 + j) * SC] * z1;
+}
+// y_i = J_i^T z
+template <int NI, int SC>
+__device__ __forceinline__ void obs_JiT(const double* ji, double z0, double z1, double y[]) {
+#pragma unroll
+  for (int j = 0; j < NI; ++j) y[j] = ji[j * SC] * z0 + ji[(NI + j) * SC] * z1;
+}
+// The observation's share of the model cost change -m.(r + m/2), model residual m = J * step = -(F xs + E u) = -(r - z).
+__device__ __forceinline__ double obs_model_cost_change(double r0, double r1, double z0, double z1) {
+  const double m0 = -(r0 - z0), m1 = -(r1 - z1);
+  return -(m0 * (r0 + 0.5 * m0) + m1 * (r1 + 0.5 * m1));
+}
+// The 21 upper-triangle entries of J_c^T Q_o J_c, Q_o = I_2 - J_p M_p J_p^T (SCHUR_JACOBI camera block).
+__device__ __forceinline__ void obs_cam_block(const double* __restrict__ M, const double ja[6], const double jh[2], const double jw[6], double h,
+                                              double v[21]) {
+  const double jp0[4] = {ja[0], ja[1], ja[2], jh[0]}, jp1[4] = {ja[3], ja[4], ja[5], jh[1]};
+  double m0[4], m1[4];
+  sym4_mul(M, jp0, m0);
+  sym4_mul(M, jp1, m1);
+  const double q00 = 1.0 - (jp0[0] * m0[0] + jp0[1] * m0[1] + jp0[2] * m0[2] + jp0[3] * m0[3]);
+  const double q01 = -(jp0[0] * m1[0] + jp0[1] * m1[1] + jp0[2] * m1[2] + jp0[3] * m1[3]);
+  const double q11 = 1.0 - (jp1[0] * m1[0] + jp1[1] * m1[1] + jp1[2] * m1[2] + jp1[3] * m1[3]);
+  double c0[6], c1[6];
+#pragma unroll
+  for (int j = 0; j < 3; ++j) { c0[j] = -h * ja[j]; c1[j] = -h * ja[3 + j]; c0[3 + j] = jw[j]; c1[3 + j] = jw[3 + j]; }
+  int n = 0;
+#pragma unroll
+  for (int a = 0; a < 6; ++a) {
+    const double qa0 = q00 * c0[a] + q01 * c1[a], qa1 = q01 * c0[a] + q11 * c1[a];
+#pragma unroll
+    for (int b = a; b < 6; ++b) { v[n] = qa0 * c0[b] + qa1 * c1[b]; ++n; }
+  }
+}
+// The NI (NI + 1) / 2 upper-triangle entries of J_i^T J_i.
+template <int NI>
+__device__ __forceinline__ void obs_JiT_Ji(const double* ji, double g[]) {
+  int n = 0;
+#pragma unroll
+  for (int a = 0; a < NI; ++a)
+#pragma unroll
+    for (int b = a; b < NI; ++b) { g[n] = ji[a] * ji[b] + ji[NI + a] * ji[NI + b]; ++n; }
+}
+// The upper triangle of W^T M_p W for one (point, group) run, W = sum_{o in the run} J_p^T J_i (4 x NI, W[a * NI + j]).
+template <int NI>
+__device__ __forceinline__ void run_WT_M_W(const double* __restrict__ M, const double* W, double sub[]) {
+  double MW[4][NI + 1];
+#pragma unroll
+  for (int j = 0; j < NI; ++j) {
+    const double t[4] = {W[0 * NI + j], W[1 * NI + j], W[2 * NI + j], W[3 * NI + j]};
+    double u[4];
+    sym4_mul(M, t, u);
+    MW[0][j] = u[0]; MW[1][j] = u[1]; MW[2][j] = u[2]; MW[3][j] = u[3];
+  }
+  int n = 0;
+#pragma unroll
+  for (int a = 0; a < NI; ++a)
+#pragma unroll
+    for (int b = a; b < NI; ++b) {
+      sub[n] = W[0 * NI + a] * MW[0][b] + W[1 * NI + a] * MW[1][b] + W[2 * NI + a] * MW[2][b] + W[3 * NI + a] * MW[3][b];
+      ++n;
+    }
+}
+// Offset of entry (ia, ib), ia <= ib, in the row-major upper triangle of a 10 x 10 block (the padded intrinsics blocks).
+__device__ __forceinline__ int tri10(int ia, int ib) { return ia * 10 - ia * (ia - 1) / 2 + (ib - ia); }
+
+// Linearisation: Ceres' bookkeeping of one observation.  A failed projection counts as a failure; one whose parameter blocks
+// are all constant goes to the fixed cost (Ceres removes the residual: fixed_cost).  Either way its rows and residual are zeroed.
+template <int NI>
+__device__ __forceinline__ void obs_settle(bool ok, bool is_fixed, double rho0, double& cost, double& fixed, double& failed, double Ja[6],
+                                           double Jw[6], double Jh[2], double Ji[], double r[2]) {
+  if (!ok) failed += 1.0;
+  else if (is_fixed) fixed += 0.5 * rho0;
+  else cost += 0.5 * rho0;
+  if (!ok || is_fixed) {
+#pragma unroll
+    for (int j = 0; j < 6; ++j) { Ja[j] = 0.0; Jw[j] = 0.0; }
+    Jh[0] = Jh[1] = 0.0; r[0] = r[1] = 0.0;
+#pragma unroll
+    for (int j = 0; j < 2 * NI; ++j) Ji[j] = 0.0;
+  }
+}
+// Stores the observation's compact rows into its warp slice (Jt, rt: the lane's element of row 0; [NJ][32] and [2][32]).
+template <int NI>
+__device__ __forceinline__ void obs_store(double* Jt, double* rt, const double Ja[6], const double Jw[6], const double Jh[2], const double Ji[],
+                                          const double r[2]) {
+#pragma unroll
+  for (int j = 0; j < 6; ++j) Jt[j * 32] = Ja[j];
+#pragma unroll
+  for (int j = 0; j < 6; ++j) Jt[(6 + j) * 32] = Jw[j];
+  Jt[12 * 32] = Jh[0];
+  Jt[13 * 32] = Jh[1];
+#pragma unroll
+  for (int j = 0; j < 2 * NI; ++j) Jt[(14 + j) * 32] = Ji[j];
+  rt[0] = r[0];
+  rt[32] = r[1];
+}
+// The observation's terms of the per-point blocks: H_pp = J_p^T J_p (acc[0..9], row-major upper), g_p = J_p^T r (acc[10..13]).
+__device__ __forceinline__ void obs_point_terms(const double Ja[6], const double Jh[2], const double r[2], double acc[14]) {
+  const double jp0[4] = {Ja[0], Ja[1], Ja[2], Jh[0]}, jp1[4] = {Ja[3], Ja[4], Ja[5], Jh[1]};
+  int n = 0;
+#pragma unroll
+  for (int a = 0; a < 4; ++a)
+#pragma unroll
+    for (int b = a; b < 4; ++b) acc[n++] = jp0[a] * jp0[b] + jp1[a] * jp1[b];
+#pragma unroll
+  for (int a = 0; a < 4; ++a) acc[10 + a] = jp0[a] * r[0] + jp1[a] * r[1];
+}
+// Camera gradient J_c^T r and squared column norms of J_c.
+__device__ __forceinline__ void obs_cam_grad(const double Ja[6], const double Jw[6], double h, const double r[2], double g[6], double cn[6]) {
+#pragma unroll
+  for (int j = 0; j < 3; ++j) {
+    const double c0 = -h * Ja[j], c1 = -h * Ja[3 + j];
+    g[j] = c0 * r[0] + c1 * r[1];
+    cn[j] = c0 * c0 + c1 * c1;
+    g[3 + j] = Jw[j] * r[0] + Jw[3 + j] * r[1];
+    cn[3 + j] = Jw[j] * Jw[j] + Jw[3 + j] * Jw[3 + j];
+  }
+}
+// Column j of the intrinsics gradient J_i^T r and of the squared column norms of J_i.
+template <int NI>
+__device__ __forceinline__ void obs_intr_grad(const double Ji[], const double r[2], int j, double& g, double& cn) {
+  g = Ji[j] * r[0] + Ji[NI + j] * r[1];
+  cn = Ji[j] * Ji[j] + Ji[NI + j] * Ji[NI + j];
+}
+
 // ---------------------------------------------------------- K1 linearise
 // One thread per observation slot.  Writes the compact linearisation and the robustified residual
 // ([tile][warp][NJ][32] / [tile][warp][2][32]: a warp's slice is contiguous), the per-point blocks, the camera-side
@@ -233,44 +400,14 @@ __global__ void __launch_bounds__(TILE, EXT ? 1 : 3) k_linearize(DevProblem P, d
     const bool ok = linearize_obs_any<IMASK, EXT>(P.group_model[grp], Cw, rec,
                                          P.intr + (size_t)grp * 10, X.x, X.y, X.z, X.w, x, y, P.loss_type, P.loss_width,
                                          r, rho0, Ja, Jw, Jh, Ji);
-    const bool is_fixed = (P.slot_flags[slot] & 1) != 0;
-    if (!ok) failed = 1.0;
-    else if (is_fixed) fixed = 0.5 * rho0;  // every block constant: Ceres removes the residual (fixed_cost)
-    else cost = 0.5 * rho0;
-    if (!ok || is_fixed) {
-#pragma unroll
-      for (int j = 0; j < 6; ++j) { Ja[j] = 0.0; Jw[j] = 0.0; }
-      Jh[0] = Jh[1] = 0.0; r[0] = r[1] = 0.0;
-#pragma unroll
-      for (int j = 0; j < 2 * NI; ++j) Ji[j] = 0.0;
-    }
+    obs_settle<NI>(ok, (P.slot_flags[slot] & 1) != 0, rho0, cost, fixed, failed, Ja, Jw, Jh, Ji, r);
   }
   // store the compact linearisation (each warp writes 256-byte rows of its own slice)
+  obs_store<NI>(P.J + wslice(tile, warp, NJ) + lane, P.res + wslice(tile, warp, 2) + lane, Ja, Jw, Jh, Ji, r);
+  // per-point blocks H_pp, g_p
   {
-    double* Jt = P.J + wslice(tile, warp, NJ) + lane;
-#pragma unroll
-    for (int j = 0; j < 6; ++j) Jt[j * 32] = Ja[j];
-#pragma unroll
-    for (int j = 0; j < 6; ++j) Jt[(6 + j) * 32] = Jw[j];
-    Jt[12 * 32] = Jh[0];
-    Jt[13 * 32] = Jh[1];
-#pragma unroll
-    for (int j = 0; j < 2 * NI; ++j) Jt[(14 + j) * 32] = Ji[j];
-    double* rt = P.res + wslice(tile, warp, 2) + lane;
-    rt[0] = r[0];
-    rt[32] = r[1];
-  }
-  // per-point blocks: H_pp = J_p^T J_p (10, row-major upper), g_p = J_p^T r with J_p = [Ja | Jh]
-  {
-    const double jp0[4] = {Ja[0], Ja[1], Ja[2], Jh[0]}, jp1[4] = {Ja[3], Ja[4], Ja[5], Jh[1]};
     double acc[14];
-    int n = 0;
-#pragma unroll
-    for (int a = 0; a < 4; ++a)
-#pragma unroll
-      for (int b = a; b < 4; ++b) acc[n++] = jp0[a] * jp0[b] + jp1[a] * jp1[b];
-#pragma unroll
-    for (int a = 0; a < 4; ++a) acc[10 + a] = jp0[a] * r[0] + jp1[a] * r[1];
+    obs_point_terms(Ja, Jh, r, acc);
     const int prev = __shfl_up_sync(0xffffffffu, pl, 1);
     const bool head = valid && (lane == 0 || prev != pl);
 #pragma unroll
@@ -289,18 +426,11 @@ __global__ void __launch_bounds__(TILE, EXT ? 1 : 3) k_linearize(DevProblem P, d
       }
     }
   }
-  // camera-side gradient and squared column norms: J_c = [-h Ja | Jw]
+  // camera-side gradient and squared column norms
+  double gv[6], cv[6];
   if (STAGED_RED && !long_tile) {
     // both 6-rows staged per warp in the (idle on normal tiles) s_acc area, emitted element-major
-    double gv[6], cv[6];
-#pragma unroll
-    for (int j = 0; j < 3; ++j) {
-      const double c0 = -h * Ja[j], c1 = -h * Ja[3 + j];
-      gv[j] = c0 * r[0] + c1 * r[1];
-      cv[j] = c0 * c0 + c1 * c1;
-      gv[3 + j] = Jw[j] * r[0] + Jw[3 + j] * r[1];
-      cv[3 + j] = Jw[j] * Jw[j] + Jw[3 + j] * Jw[3 + j];
-    }
+    obs_cam_grad(Ja, Jw, h, r, gv, cv);
     static_assert(MAXP * 14 >= (TILE / 32) * (2 * 32 * 6 + 16), "s_acc too small for the row staging");
     double* stage = &s_acc[0][0] + warp * (2 * 32 * 6 + 16);
     int* sbase = reinterpret_cast<int*>(stage + 2 * 32 * 6);
@@ -310,34 +440,30 @@ __global__ void __launch_bounds__(TILE, EXT ? 1 : 3) k_linearize(DevProblem P, d
     warp_red_rows<6>(g_cs, stage, sbase, lane);
     warp_red_rows<6>(cn_cs, stage + 32 * 6, sbase, lane);
   } else if (valid) {
-    double* gc = g_cs + (size_t)cam * 6;
-    double* cc = cn_cs + (size_t)cam * 6;
+    obs_cam_grad(Ja, Jw, h, r, gv, cv);
 #pragma unroll
-    for (int j = 0; j < 3; ++j) {
-      const double c0 = -h * Ja[j], c1 = -h * Ja[3 + j];
-      red_add(gc + j, c0 * r[0] + c1 * r[1]);
-      red_add(cc + j, c0 * c0 + c1 * c1);
-    }
-#pragma unroll
-    for (int j = 0; j < 3; ++j) {
-      red_add(gc + 3 + j, Jw[j] * r[0] + Jw[3 + j] * r[1]);
-      red_add(cc + 3 + j, Jw[j] * Jw[j] + Jw[3 + j] * Jw[3 + j]);
+    for (int j = 0; j < 6; ++j) {
+      red_add(g_cs + (size_t)cam * 6 + j, gv[j]);
+      red_add(cn_cs + (size_t)cam * 6 + j, cv[j]);
     }
   }
   double* rr = rep_row(rep);
   if (NI > 0) {
+    double g, c;
     if (P.single_group) {
 #pragma unroll
       for (int j = 0; j < NI; ++j) {
-        const double gsum = warp_sum(Ji[j] * r[0] + Ji[NI + j] * r[1]);
-        const double csum = warp_sum(Ji[j] * Ji[j] + Ji[NI + j] * Ji[NI + j]);
+        obs_intr_grad<NI>(Ji, r, j, g, c);
+        const double gsum = warp_sum(g);
+        const double csum = warp_sum(c);
         if (lane == 0) { red_add(rr + nth_bit(IMASK, j), gsum); red_add(rr + 10 + nth_bit(IMASK, j), csum); }
       }
     } else if (valid) {
 #pragma unroll
       for (int j = 0; j < NI; ++j) {
-        red_add(g_cs + P.ne + (size_t)grp * 10 + nth_bit(IMASK, j), Ji[j] * r[0] + Ji[NI + j] * r[1]);
-        red_add(cn_cs + P.ne + (size_t)grp * 10 + nth_bit(IMASK, j), Ji[j] * Ji[j] + Ji[NI + j] * Ji[NI + j]);
+        obs_intr_grad<NI>(Ji, r, j, g, c);
+        red_add(g_cs + P.ne + (size_t)grp * 10 + nth_bit(IMASK, j), g);
+        red_add(cn_cs + P.ne + (size_t)grp * 10 + nth_bit(IMASK, j), c);
       }
     }
   }
@@ -597,13 +723,6 @@ __global__ void k_point_blocks(DevProblem P, double radius, double lo, double hi
     for (int b = a; b < 4; ++b) { M[n] = s[a] * Ai[n] * s[b]; ++n; }
 }
 
-__device__ __forceinline__ void sym4_mul(const double* __restrict__ M, const double t[4], double u[4]) {
-  u[0] = M[0] * t[0] + M[1] * t[1] + M[2] * t[2] + M[3] * t[3];
-  u[1] = M[1] * t[0] + M[4] * t[1] + M[5] * t[2] + M[6] * t[3];
-  u[2] = M[2] * t[0] + M[5] * t[1] + M[7] * t[2] + M[8] * t[3];
-  u[3] = M[3] * t[0] + M[6] * t[1] + M[8] * t[2] + M[9] * t[3];
-}
-
 // ---------------------------------------------------- TMA (bulk async copy) helpers
 #ifdef TBA_EMULATE
 // CPU emulation build (tests/emu/cuda_emu.h): the bulk copy is a memcpy by the issuing lane, the mbarrier a flag the other lanes
@@ -723,29 +842,18 @@ __global__ void __launch_bounds__(TILE, (14 + 2 * popcount10(IMASK)) <= 20 ? 4 :
   const bool head = lane == 0 || prev != pl;
   __syncthreads();  // s_t zeroed
   mbar_wait(&s_bar[warp], 0);  // this warp's slice landed in shared memory
-  const double* Jt = sJ + lane;
-#define JA(j) Jt[(j) * 32]
-#define JW(j) Jt[(6 + (j)) * 32]
-#define JH(j) Jt[(12 + (j)) * 32]
-#define JI(j) Jt[(14 + (j)) * 32]
+  // the lane's rows in the stage (stride 32)
+  const double *ja = sJ + lane, *jw = ja + 6 * 32, *jh = ja + 12 * 32, *ji = ja + 14 * 32;
   double w0 = 0.0, w1 = 0.0, r0 = 0.0, r1 = 0.0;
   if (valid) {
     if (MODE != 0) { r0 = sR[lane]; r1 = sR[32 + lane]; }
-    if (MODE != 1) {
-      w0 = -h * (JA(0) * xa.x + JA(1) * xa.y + JA(2) * xb.x) + JW(0) * xb.y + JW(1) * xc.x + JW(2) * xc.y;
-      w1 = -h * (JA(3) * xa.x + JA(4) * xa.y + JA(5) * xb.x) + JW(3) * xb.y + JW(4) * xc.x + JW(5) * xc.y;
-#pragma unroll
-      for (int j = 0; j < NI; ++j) { w0 += JI(j) * xi[j]; w1 += JI(NI + j) * xi[j]; }
-    }
+    if (MODE != 1) obs_apply_F<NI, 32, 32>(ja, jw, ji, h, xa, xb, xc, xi, w0, w1);
     if (MODE == 1) { w0 = r0; w1 = r1; }
     if (MODE == 2) { w0 = r0 - w0; w1 = r1 - w1; }
   }
-  // t_p = sum_o J_p^T w,  J_p = [Ja | Jh]
+  // t_p = sum_o J_p^T w
   double t[4] = {0.0, 0.0, 0.0, 0.0};
-  if (valid) {
-    t[0] = JA(0) * w0 + JA(3) * w1; t[1] = JA(1) * w0 + JA(4) * w1; t[2] = JA(2) * w0 + JA(5) * w1;
-    t[3] = JH(0) * w0 + JH(1) * w1;
-  }
+  if (valid) obs_JpT<32>(ja, jh, w0, w1, t);
 #pragma unroll
   for (int j = 0; j < 4; ++j) t[j] = seg_reduce(t[j], pl, lane);
   if (head && valid) {
@@ -764,33 +872,25 @@ __global__ void __launch_bounds__(TILE, (14 + 2 * popcount10(IMASK)) <= 20 ? 4 :
     }
   }
   __syncthreads();
-  double u0 = 0.0, u1 = 0.0, u2 = 0.0, u3 = 0.0;
-  if (valid) { u0 = s_t[pl][0]; u1 = s_t[pl][1]; u2 = s_t[pl][2]; u3 = s_t[pl][3]; }
+  double u[4] = {0.0, 0.0, 0.0, 0.0};
+  if (valid) { u[0] = s_t[pl][0]; u[1] = s_t[pl][1]; u[2] = s_t[pl][2]; u[3] = s_t[pl][3]; }
   double z0 = 0.0, z1 = 0.0;
-  if (valid) {
-    z0 = w0 - (JA(0) * u0 + JA(1) * u1 + JA(2) * u2 + JH(0) * u3);
-    z1 = w1 - (JA(3) * u0 + JA(4) * u1 + JA(5) * u2 + JH(1) * u3);
-  }
+  if (valid) obs_sub_Jp<32>(ja, jh, w0, w1, u, z0, z1);
   double* rr = rep_row(rep);
   if (MODE == 2) {
-    // model residual m = J * step = -(F xs + E u) = -(r - z); contribution -m.(r + m/2)
     double mcc = 0.0;
-    if (valid && !(P.slot_flags[slot] & 1)) {
-      const double m0 = -(r0 - z0), m1 = -(r1 - z1);
-      mcc = -(m0 * (r0 + 0.5 * m0) + m1 * (r1 + 0.5 * m1));
-    }
+    if (valid && !(P.slot_flags[slot] & 1)) mcc = obs_model_cost_change(r0, r1, z0, z1);
     mcc = warp_sum(mcc);
     if (lane == 0) red_add(rr + 23, mcc);
   } else {
     // camera-side contributions staged per warp and emitted element-major (warp_red_rows)
-    double yv[6];
+    double yv[6], yi[NI + 1];
+    obs_JcT<32, 32>(ja, jw, h, z0, z1, yv);
+    obs_JiT<NI, 32>(ji, z0, z1, yi);
 #pragma unroll
-    for (int j = 0; j < 3; ++j) yv[j] = valid ? -h * (JA(j) * z0 + JA(3 + j) * z1) : 0.0;
+    for (int j = 0; j < 6; ++j) yv[j] = valid ? yv[j] : 0.0;
 #pragma unroll
-    for (int j = 0; j < 3; ++j) yv[3 + j] = valid ? JW(j) * z0 + JW(3 + j) * z1 : 0.0;
-    double yi[NI + 1];
-#pragma unroll
-    for (int j = 0; j < NI; ++j) yi[j] = valid ? JI(j) * z0 + JI(NI + j) * z1 : 0.0;
+    for (int j = 0; j < NI; ++j) yi[j] = valid ? yi[j] : 0.0;
     __syncwarp();  // every lane has finished reading the J slice: its first 6.5 rows are reused as staging [32][6] + 32 ints
     int* sbase = reinterpret_cast<int*>(sJ + 32 * 6);
     warp_stage_row<6>(sJ, sbase, yv, valid ? cam * 6 : -1, lane);
@@ -809,10 +909,6 @@ __global__ void __launch_bounds__(TILE, (14 + 2 * popcount10(IMASK)) <= 20 ? 4 :
       }
     }
   }
-#undef JA
-#undef JW
-#undef JH
-#undef JI
 }
 
 // --------------------------------------------- fused matvec + all-reduce over NVLink peer memory (multi-GPU)
@@ -1021,71 +1117,52 @@ k_schur_stream(DevProblem P, const double* __restrict__ xs, double* __restrict__
     const int stage = it % NS;
     double* sJ = ring + (size_t)stage * STG;
     const double* sR = sJ + NJ * 32;
-    const double* Jt = sJ + lane;
-#define JA(j) Jt[(j) * 32]
-#define JW(j) Jt[(6 + (j)) * 32]
-#define JH(j) Jt[(12 + (j)) * 32]
-#define JI(j) Jt[(14 + (j)) * 32]
+    // J_a and J_h of this lane in registers (every element read from shared memory exactly once), J_w and J_i in the stage
+    const double *jw = sJ + lane + 6 * 32, *ji = sJ + lane + 14 * 32;
     double w0 = 0.0, w1 = 0.0, r0 = 0.0, r1 = 0.0;
-    // the whole row set of this lane in registers: every element of J is read from shared memory exactly once
     double ja[6], jh[2];
 #pragma unroll
-    for (int j = 0; j < 6; ++j) ja[j] = JA(j);
-    jh[0] = JH(0); jh[1] = JH(1);
+    for (int j = 0; j < 6; ++j) ja[j] = sJ[j * 32 + lane];
+    jh[0] = sJ[12 * 32 + lane]; jh[1] = sJ[13 * 32 + lane];
     if (valid) {
       if (MODE != 0) { r0 = sR[lane]; r1 = sR[32 + lane]; }
-      if (MODE != 1) {
-        w0 = -h * (ja[0] * xa.x + ja[1] * xa.y + ja[2] * xb.x) + JW(0) * xb.y + JW(1) * xc.x + JW(2) * xc.y;
-        w1 = -h * (ja[3] * xa.x + ja[4] * xa.y + ja[5] * xb.x) + JW(3) * xb.y + JW(4) * xc.x + JW(5) * xc.y;
-#pragma unroll
-        for (int j = 0; j < NI; ++j) { w0 += JI(j) * xi[j]; w1 += JI(NI + j) * xi[j]; }
-      }
+      if (MODE != 1) obs_apply_F<NI, 1, 32>(ja, jw, ji, h, xa, xb, xc, xi, w0, w1);
       if (MODE == 1) { w0 = r0; w1 = r1; }
       if (MODE == 2) { w0 = r0 - w0; w1 = r1 - w1; }
     }
     double t[4] = {0.0, 0.0, 0.0, 0.0};
-    if (valid) {
-      t[0] = ja[0] * w0 + ja[3] * w1; t[1] = ja[1] * w0 + ja[4] * w1; t[2] = ja[2] * w0 + ja[5] * w1;
-      t[3] = jh[0] * w0 + jh[1] * w1;
-    }
+    if (valid) obs_JpT<1>(ja, jh, w0, w1, t);
     if (!(MODE == 0 && (P.ablate & 8))) {
       const int last = run_last_lane_dev(heads, lane);
 #pragma unroll
       for (int j = 0; j < 4; ++j) t[j] = seg_reduce_to(t[j], last, lane);
     }
-    double u0 = m01.x * t[0] + m01.y * t[1] + m23.x * t[2] + m23.y * t[3];
-    double u1 = m01.y * t[0] + m45.x * t[1] + m45.y * t[2] + m67.x * t[3];
-    double u2 = m23.x * t[0] + m45.y * t[1] + m67.y * t[2] + m89.x * t[3];
-    double u3 = m23.y * t[0] + m67.x * t[1] + m89.x * t[2] + m89.y * t[3];
+    double u[4];
+    u[0] = m01.x * t[0] + m01.y * t[1] + m23.x * t[2] + m23.y * t[3];
+    u[1] = m01.y * t[0] + m45.x * t[1] + m45.y * t[2] + m67.x * t[3];
+    u[2] = m23.x * t[0] + m45.y * t[1] + m67.y * t[2] + m89.x * t[3];
+    u[3] = m23.y * t[0] + m67.x * t[1] + m89.x * t[2] + m89.y * t[3];
     const bool head = (heads >> lane) & 1u;
     if (MODE == 2 && head && valid) {
       double2* d = reinterpret_cast<double2*>(P.dpt + (size_t)pt * 4);
-      d[0] = make_double2(-u0, -u1);
-      d[1] = make_double2(-u2, -u3);
+      d[0] = make_double2(-u[0], -u[1]);
+      d[1] = make_double2(-u[2], -u[3]);
     }
     const int hl = run_head_lane(heads, lane);
-    u0 = __shfl_sync(0xffffffffu, u0, hl); u1 = __shfl_sync(0xffffffffu, u1, hl);
-    u2 = __shfl_sync(0xffffffffu, u2, hl); u3 = __shfl_sync(0xffffffffu, u3, hl);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) u[j] = __shfl_sync(0xffffffffu, u[j], hl);
     double z0 = 0.0, z1 = 0.0;
-    if (valid) {
-      z0 = w0 - (ja[0] * u0 + ja[1] * u1 + ja[2] * u2 + jh[0] * u3);
-      z1 = w1 - (ja[3] * u0 + ja[4] * u1 + ja[5] * u2 + jh[1] * u3);
-    }
+    if (valid) obs_sub_Jp<1>(ja, jh, w0, w1, u, z0, z1);
     if (MODE == 2) {
-      // model residual m = J * step = -(F xs + E u) = -(r - z); contribution -m.(r + m/2)
-      if (valid && !(flag & 1)) {
-        const double m0 = -(r0 - z0), m1 = -(r1 - z1);
-        mcc_acc += -(m0 * (r0 + 0.5 * m0) + m1 * (r1 + 0.5 * m1));
-      }
+      if (valid && !(flag & 1)) mcc_acc += obs_model_cost_change(r0, r1, z0, z1);
     } else {
-      double yv[6];
+      double yv[6], yi[NI + 1];
+      obs_JcT<1, 32>(ja, jw, h, z0, z1, yv);
+      obs_JiT<NI, 32>(ji, z0, z1, yi);
 #pragma unroll
-      for (int j = 0; j < 3; ++j) yv[j] = valid ? -h * (ja[j] * z0 + ja[3 + j] * z1) : 0.0;
+      for (int j = 0; j < 6; ++j) yv[j] = valid ? yv[j] : 0.0;
 #pragma unroll
-      for (int j = 0; j < 3; ++j) yv[3 + j] = valid ? JW(j) * z0 + JW(3 + j) * z1 : 0.0;
-      double yi[NI + 1];
-#pragma unroll
-      for (int j = 0; j < NI; ++j) yi[j] = valid ? JI(j) * z0 + JI(NI + j) * z1 : 0.0;
+      for (int j = 0; j < NI; ++j) yi[j] = valid ? yi[j] : 0.0;
       __syncwarp();  // every lane has finished reading the J slice: its first rows are reused as staging [32][6] + 32 ints
       int* sbase = reinterpret_cast<int*>(sJ + 32 * 6);
       warp_stage_row<6>(sJ, sbase, yv, valid ? cam * 6 : -1, lane);
@@ -1109,10 +1186,6 @@ k_schur_stream(DevProblem P, const double* __restrict__ xs, double* __restrict__
         }
       }
     }
-#undef JA
-#undef JW
-#undef JH
-#undef JI
     // ---- the stage is consumed: re-arm it for slice s + NS
     __syncwarp();
     if (lane == 0 && s + NS < s_end) {
@@ -1296,18 +1369,18 @@ k_prepare_stream(DevProblem P, double* __restrict__ y, double* __restrict__ Sc, 
     const int hl = run_head_lane(heads, lane);
     // ---------------- reduced rhs (MODE 1 of k_schur): w = r
     {
-      double t[4] = {ja[0] * r0 + ja[3] * r1, ja[1] * r0 + ja[4] * r1, ja[2] * r0 + ja[5] * r1, jh[0] * r0 + jh[1] * r1};
+      double t[4];
+      obs_JpT<1>(ja, jh, r0, r1, t);
 #pragma unroll
       for (int j = 0; j < 4; ++j) t[j] = seg_reduce_to(t[j], last, lane);
       double u[4];
       sym4_mul(M, t, u);
 #pragma unroll
       for (int j = 0; j < 4; ++j) u[j] = __shfl_sync(0xffffffffu, u[j], hl);
-      const double z0 = r0 - (ja[0] * u[0] + ja[1] * u[1] + ja[2] * u[2] + jh[0] * u[3]);
-      const double z1 = r1 - (ja[3] * u[0] + ja[4] * u[1] + ja[5] * u[2] + jh[1] * u[3]);
-      double yv[6];
-#pragma unroll
-      for (int j = 0; j < 3; ++j) { yv[j] = -h * (ja[j] * z0 + ja[3 + j] * z1); yv[3 + j] = jw[j] * z0 + jw[3 + j] * z1; }
+      double z0, z1, yv[6], yi[NI + 1];
+      obs_sub_Jp<1>(ja, jh, r0, r1, u, z0, z1);
+      obs_JcT<1, 1>(ja, jw, h, z0, z1, yv);
+      obs_JiT<NI, 1>(ji, z0, z1, yi);
       int* sbase = reinterpret_cast<int*>(sJ + 32 * 6);
       warp_stage_row<6>(sJ, sbase, yv, valid ? cam * 6 : -1, lane);
       __syncwarp();
@@ -1315,34 +1388,18 @@ k_prepare_stream(DevProblem P, double* __restrict__ y, double* __restrict__ Sc, 
       if (NI > 0) {
         if (P.single_group) {
 #pragma unroll
-          for (int j = 0; j < NI; ++j) yi_acc[j] += ji[j] * z0 + ji[NI + j] * z1;
+          for (int j = 0; j < NI; ++j) yi_acc[j] += yi[j];
         } else if (valid) {
 #pragma unroll
-          for (int j = 0; j < NI; ++j) red_add(y + P.ne + (size_t)grp * 10 + nth_bit(IMASK, j), ji[j] * z0 + ji[NI + j] * z1);
+          for (int j = 0; j < NI; ++j) red_add(y + P.ne + (size_t)grp * 10 + nth_bit(IMASK, j), yi[j]);
         }
       }
       __syncwarp();
     }
     // ---------------- extrinsics blocks: 21 entries per observation, staged and emitted in three groups of seven columns
     {
-      const double jp0[4] = {ja[0], ja[1], ja[2], jh[0]}, jp1[4] = {ja[3], ja[4], ja[5], jh[1]};
-      double m0[4], m1[4];
-      sym4_mul(M, jp0, m0);
-      sym4_mul(M, jp1, m1);
-      const double q00 = 1.0 - (jp0[0] * m0[0] + jp0[1] * m0[1] + jp0[2] * m0[2] + jp0[3] * m0[3]);
-      const double q01 = -(jp0[0] * m1[0] + jp0[1] * m1[1] + jp0[2] * m1[2] + jp0[3] * m1[3]);
-      const double q11 = 1.0 - (jp1[0] * m1[0] + jp1[1] * m1[1] + jp1[2] * m1[2] + jp1[3] * m1[3]);
-      double c0[6], c1[6];
-#pragma unroll
-      for (int j = 0; j < 3; ++j) { c0[j] = -h * ja[j]; c1[j] = -h * ja[3 + j]; c0[3 + j] = jw[j]; c1[3 + j] = jw[3 + j]; }
       double v[21];
-      int n = 0;
-#pragma unroll
-      for (int a = 0; a < 6; ++a) {
-        const double qa0 = q00 * c0[a] + q01 * c1[a], qa1 = q01 * c0[a] + q11 * c1[a];
-#pragma unroll
-        for (int b = a; b < 6; ++b) { v[n] = qa0 * c0[b] + qa1 * c1[b]; ++n; }
-      }
+      obs_cam_block(M, ja, jh, jw, h, v);
       int* sbase = reinterpret_cast<int*>(sJ + 32 * 7);
 #pragma unroll
       for (int g3 = 0; g3 < 3; ++g3) {
@@ -1365,39 +1422,18 @@ k_prepare_stream(DevProblem P, double* __restrict__ y, double* __restrict__ Sc, 
 #pragma unroll
         for (int j = 0; j < NI; ++j) W[a * NI + j] = seg_reduce_to(p0 * ji[j] + p1 * ji[NI + j], rlast, lane);
       }
-      double sub[NSI + 1];
+      double sub[NSI + 1], acc[NSI + 1];
 #pragma unroll
       for (int j = 0; j < NSI; ++j) sub[j] = 0.0;
-      if (rhead && valid) {
-        double MW[4][NI + 1];
-#pragma unroll
-        for (int j = 0; j < NI; ++j) {
-          const double t4[4] = {W[0 * NI + j], W[1 * NI + j], W[2 * NI + j], W[3 * NI + j]};
-          double u4[4];
-          sym4_mul(M, t4, u4);
-          MW[0][j] = u4[0]; MW[1][j] = u4[1]; MW[2][j] = u4[2]; MW[3][j] = u4[3];
-        }
-        int n = 0;
-#pragma unroll
-        for (int a = 0; a < NI; ++a)
-#pragma unroll
-          for (int b = a; b < NI; ++b) {
-            sub[n] = W[0 * NI + a] * MW[0][b] + W[1 * NI + a] * MW[1][b] + W[2 * NI + a] * MW[2][b] + W[3 * NI + a] * MW[3][b];
-            ++n;
-          }
-      }
+      if (rhead && valid) run_WT_M_W<NI>(M, W, sub);
+      obs_JiT_Ji<NI>(ji, acc);  // 0 on padding lanes
       int n = 0;
 #pragma unroll
       for (int a = 0; a < NI; ++a)
 #pragma unroll
         for (int b = a; b < NI; ++b) {
-          const double acc = ji[a] * ji[b] + ji[NI + a] * ji[NI + b];  // 0 on padding lanes
-          if (P.single_group) si_acc[n] += acc - sub[n];
-          else if (valid) {
-            const int ia = nth_bit(IMASK, a), ib = nth_bit(IMASK, b);
-            const int idx = ia * 10 - ia * (ia - 1) / 2 + (ib - ia);
-            red_add(Si + (size_t)grp * 55 + idx, acc - sub[n]);
-          }
+          if (P.single_group) si_acc[n] += acc[n] - sub[n];
+          else if (valid) red_add(Si + (size_t)grp * 55 + tri10(nth_bit(IMASK, a), nth_bit(IMASK, b)), acc[n] - sub[n]);
           ++n;
         }
     }
@@ -1428,7 +1464,7 @@ k_prepare_stream(DevProblem P, double* __restrict__ y, double* __restrict__ Sc, 
       int n = 0, idx = 0;
       for (int a = 0; a < NI; ++a)
         for (int b = a; b < NI; ++b) {
-          if (n == (int)threadIdx.x) { const int ia = nth_bit(IMASK, a), ib = nth_bit(IMASK, b); idx = ia * 10 - ia * (ia - 1) / 2 + (ib - ia); }
+          if (n == (int)threadIdx.x) idx = tri10(nth_bit(IMASK, a), nth_bit(IMASK, b));
           ++n;
         }
       red_add(Si + idx, vsum);
@@ -1556,43 +1592,14 @@ k_linearize_stream(DevProblem P, double* __restrict__ g_cs, double* __restrict__
       double rho0 = 0.0;
       const bool ok = linearize_obs_any<IMASK, false>(P.group_model[grp], Cw, rec, P.intr + (size_t)grp * 10, X01.x, X01.y, X23.x,
                                                       X23.y, st[lane], st[32 + lane], P.loss_type, P.loss_width, r, rho0, Ja, Jw, Jh, Ji);
-      const bool is_fixed = (reinterpret_cast<const uint8_t*>(st + 96)[lane] & 1) != 0;
-      if (!ok) failed_acc += 1.0;
-      else if (is_fixed) fixed_acc += 0.5 * rho0;  // every block constant: Ceres removes the residual (fixed_cost)
-      else cost_acc += 0.5 * rho0;
-      if (!ok || is_fixed) {
-#pragma unroll
-        for (int j = 0; j < 6; ++j) { Ja[j] = 0.0; Jw[j] = 0.0; }
-        Jh[0] = Jh[1] = 0.0; r[0] = r[1] = 0.0;
-#pragma unroll
-        for (int j = 0; j < 2 * NI; ++j) Ji[j] = 0.0;
-      }
+      obs_settle<NI>(ok, (reinterpret_cast<const uint8_t*>(st + 96)[lane] & 1) != 0, rho0, cost_acc, fixed_acc, failed_acc, Ja, Jw, Jh,
+                     Ji, r);
     }
+    obs_store<NI>(P.J + (size_t)s * NJ * 32 + lane, P.res + (size_t)s * 64 + lane, Ja, Jw, Jh, Ji, r);
+    // per-point blocks H_pp, g_p
     {
-      double* Jt = P.J + (size_t)s * NJ * 32 + lane;
-#pragma unroll
-      for (int j = 0; j < 6; ++j) Jt[j * 32] = Ja[j];
-#pragma unroll
-      for (int j = 0; j < 6; ++j) Jt[(6 + j) * 32] = Jw[j];
-      Jt[12 * 32] = Jh[0];
-      Jt[13 * 32] = Jh[1];
-#pragma unroll
-      for (int j = 0; j < 2 * NI; ++j) Jt[(14 + j) * 32] = Ji[j];
-      double* rt = P.res + (size_t)s * 64 + lane;
-      rt[0] = r[0];
-      rt[32] = r[1];
-    }
-    // per-point blocks: H_pp = J_p^T J_p (10, row-major upper), g_p = J_p^T r with J_p = [Ja | Jh]
-    {
-      const double jp0[4] = {Ja[0], Ja[1], Ja[2], Jh[0]}, jp1[4] = {Ja[3], Ja[4], Ja[5], Jh[1]};
       double acc[14];
-      int n = 0;
-#pragma unroll
-      for (int a = 0; a < 4; ++a)
-#pragma unroll
-        for (int b = a; b < 4; ++b) acc[n++] = jp0[a] * jp0[b] + jp1[a] * jp1[b];
-#pragma unroll
-      for (int a = 0; a < 4; ++a) acc[10 + a] = jp0[a] * r[0] + jp1[a] * r[1];
+      obs_point_terms(Ja, Jh, r, acc);
       const int last = run_last_lane_dev(heads, lane);
 #pragma unroll
       for (int j = 0; j < 14; ++j) acc[j] = seg_reduce_to(acc[j], last, lane);
@@ -1605,18 +1612,10 @@ k_linearize_stream(DevProblem P, double* __restrict__ g_cs, double* __restrict__
         G2[1] = make_double2(acc[12], acc[13]);
       }
     }
-    // camera-side gradient and squared column norms: J_c = [-h Ja | Jw]
+    // camera-side gradient and squared column norms
     {
-      const double h = X23.y;
       double gv[6], cv[6];
-#pragma unroll
-      for (int j = 0; j < 3; ++j) {
-        const double c0 = -h * Ja[j], c1 = -h * Ja[3 + j];
-        gv[j] = c0 * r[0] + c1 * r[1];
-        cv[j] = c0 * c0 + c1 * c1;
-        gv[3 + j] = Jw[j] * r[0] + Jw[3 + j] * r[1];
-        cv[3 + j] = Jw[j] * Jw[j] + Jw[3 + j] * Jw[3 + j];
-      }
+      obs_cam_grad(Ja, Jw, X23.y, r, gv, cv);
       __syncwarp();  // the previous slice's emission has read the staging rows
       warp_stage_row<6>(rows, rbase, gv, valid ? cam * 6 : -1, lane);
       warp_stage_row<6>(rows + 32 * 6, rbase, cv, valid ? cam * 6 : -1, lane);
@@ -1625,17 +1624,20 @@ k_linearize_stream(DevProblem P, double* __restrict__ g_cs, double* __restrict__
       warp_red_rows<6>(cn_cs, rows + 32 * 6, rbase, lane);
     }
     if (NI > 0) {
+      double g, c;
       if (P.single_group) {
 #pragma unroll
         for (int j = 0; j < NI; ++j) {
-          gi_acc[j] += Ji[j] * r[0] + Ji[NI + j] * r[1];
-          ci_acc[j] += Ji[j] * Ji[j] + Ji[NI + j] * Ji[NI + j];
+          obs_intr_grad<NI>(Ji, r, j, g, c);
+          gi_acc[j] += g;
+          ci_acc[j] += c;
         }
       } else if (valid) {
 #pragma unroll
         for (int j = 0; j < NI; ++j) {
-          red_add(g_cs + P.ne + (size_t)grp * 10 + nth_bit(IMASK, j), Ji[j] * r[0] + Ji[NI + j] * r[1]);
-          red_add(cn_cs + P.ne + (size_t)grp * 10 + nth_bit(IMASK, j), Ji[j] * Ji[j] + Ji[NI + j] * Ji[NI + j]);
+          obs_intr_grad<NI>(Ji, r, j, g, c);
+          red_add(g_cs + P.ne + (size_t)grp * 10 + nth_bit(IMASK, j), g);
+          red_add(cn_cs + P.ne + (size_t)grp * 10 + nth_bit(IMASK, j), c);
         }
       }
     }
@@ -1691,25 +1693,7 @@ __global__ void __launch_bounds__(TILE) k_precond_ext(DevProblem P, double* __re
     Jh[0] = Jt[12 * 32];
     Jh[1] = Jt[13 * 32];
     const int pt = P.slot_pt[slot];
-    const double h = P.pt[(size_t)pt * 4 + 3];
-    const double* M = P.Mp + (size_t)pt * 10;
-    const double jp0[4] = {Ja[0], Ja[1], Ja[2], Jh[0]}, jp1[4] = {Ja[3], Ja[4], Ja[5], Jh[1]};
-    double m0[4], m1[4];
-    sym4_mul(M, jp0, m0);
-    sym4_mul(M, jp1, m1);
-    const double q00 = 1.0 - (jp0[0] * m0[0] + jp0[1] * m0[1] + jp0[2] * m0[2] + jp0[3] * m0[3]);
-    const double q01 = -(jp0[0] * m1[0] + jp0[1] * m1[1] + jp0[2] * m1[2] + jp0[3] * m1[3]);
-    const double q11 = 1.0 - (jp1[0] * m1[0] + jp1[1] * m1[1] + jp1[2] * m1[2] + jp1[3] * m1[3]);
-    double c0[6], c1[6];
-#pragma unroll
-    for (int j = 0; j < 3; ++j) { c0[j] = -h * Ja[j]; c1[j] = -h * Ja[3 + j]; c0[3 + j] = Jw[j]; c1[3 + j] = Jw[3 + j]; }
-    int n = 0;
-#pragma unroll
-    for (int a = 0; a < 6; ++a) {
-      const double qa0 = q00 * c0[a] + q01 * c1[a], qa1 = q01 * c0[a] + q11 * c1[a];
-#pragma unroll
-      for (int b = a; b < 6; ++b) { v[n] = qa0 * c0[b] + qa1 * c1[b]; ++n; }
-    }
+    obs_cam_block(P.Mp + (size_t)pt * 10, Ja, Jh, Jw, P.pt[(size_t)pt * 4 + 3], v);
   }
   warp_stage_row<21>(s_stage[warp], s_base[warp], v, cam >= 0 ? cam * 21 : -1, lane);
   __syncwarp();
@@ -1763,11 +1747,7 @@ __global__ void __launch_bounds__(TILE) k_precond_intr(DevProblem P, double* __r
 #pragma unroll
         for (int j = 0; j < NI; ++j) atomicAdd(W + a * NI + j, jp0[a] * Ji[j] + jp1[a] * Ji[NI + j]);
     }
-    int n = 0;
-#pragma unroll
-    for (int a = 0; a < NI; ++a)
-#pragma unroll
-      for (int b = a; b < NI; ++b) { acc[n] = Ji[a] * Ji[b] + Ji[NI + a] * Ji[NI + b]; ++n; }
+    obs_JiT_Ji<NI>(Ji, acc);
   }
   __syncthreads();
   // per-run Schur term, handled by thread `run`
@@ -1778,24 +1758,7 @@ __global__ void __launch_bounds__(TILE) k_precond_intr(DevProblem P, double* __r
   const bool has_run = tid < nruns;
   if (has_run) {
     rgrp = s_grp[tid];
-    const double* W = s_w + (size_t)tid * NW;
-    const double* M = P.Mp + (size_t)s_pt[tid] * 10;
-    double MW[4][NI + 1];
-#pragma unroll
-    for (int j = 0; j < NI; ++j) {
-      const double t[4] = {W[0 * NI + j], W[1 * NI + j], W[2 * NI + j], W[3 * NI + j]};
-      double u[4];
-      sym4_mul(M, t, u);
-      MW[0][j] = u[0]; MW[1][j] = u[1]; MW[2][j] = u[2]; MW[3][j] = u[3];
-    }
-    int n = 0;
-#pragma unroll
-    for (int a = 0; a < NI; ++a)
-#pragma unroll
-      for (int b = a; b < NI; ++b) {
-        sub[n] = W[0 * NI + a] * MW[0][b] + W[1 * NI + a] * MW[1][b] + W[2 * NI + a] * MW[2][b] + W[3 * NI + a] * MW[3][b];
-        ++n;
-      }
+    run_WT_M_W<NI>(P.Mp + (size_t)s_pt[tid] * 10, s_w + (size_t)tid * NW, sub);
   }
   // accumulate into Si at padded parameter indices
   int n = 0;
@@ -1803,8 +1766,7 @@ __global__ void __launch_bounds__(TILE) k_precond_intr(DevProblem P, double* __r
   for (int a = 0; a < NI; ++a)
 #pragma unroll
     for (int b = a; b < NI; ++b) {
-      const int ia = nth_bit(IMASK, a), ib = nth_bit(IMASK, b);
-      const int idx = ia * 10 - ia * (ia - 1) / 2 + (ib - ia);  // upper-triangle offset in a 10x10
+      const int idx = tri10(nth_bit(IMASK, a), nth_bit(IMASK, b));
       if (P.single_group) {
         const double v = block_sum(acc[n] - sub[n], s_red);
         if (tid == 0) red_add(Si + idx, v);
