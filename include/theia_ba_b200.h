@@ -363,6 +363,11 @@ int tba_debug_linearize(tba_context* ctx, double* cost);
  * sizes_out = {n_slots, NJ, n_pt, ncs}; with any output pointer NULL only the sizes are returned. */
 int tba_debug_linearize_raw(tba_context* ctx, int tile_kernel, int64_t* sizes_out, double* J, double* res, double* Hpp,
                             double* gp, double* lin);
+/* The intrinsics columns J_i of every observation slot as the passes over the stored linearisation see them (rebuilt from the
+ * normalised image point in the compact layout, the stored rows otherwise), from the last linearisation:
+ * Ji [n_slots/32][2 NI][32], in the order of the rows 14.. of J in the full layout.  sizes_out = {n_slots, NI}; with Ji NULL only
+ * the sizes are returned. */
+int tba_debug_intr_cols(tba_context* ctx, int64_t* sizes_out, double* Ji);
 /* Launch geometry of the persistent warp-slice kernels over the normal tiles of the uploaded problem (no launch):
  * out[16] = {n_sm, n_slices, imask, has_ext_models, then {grid, warps per CTA, ring stages} of k_linearize_stream,
  * k_prepare_stream, k_schur_stream MODE 0 (matvec) and k_schur_stream MODE 1 / 2 (reduced rhs, back-substitution)}.

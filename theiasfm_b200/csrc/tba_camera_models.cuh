@@ -174,15 +174,96 @@ __host__ __device__ inline bool reproject(int model, const double* __restrict__ 
   return true;
 }
 
+// Explicitly rounded product, sum and fused multiply-add: what obs_intr_cols computes with them does not depend on how the compiler
+// contracts the code around each call site.
+__host__ __device__ inline double mul_rn(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __dmul_rn(a, b);
+#else
+  return a * b;  // only ever an operand of add_rn / fma_rn below, so no sum is left to contract it into
+#endif
+}
+__host__ __device__ inline double add_rn(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __dadd_rn(a, b);
+#else
+  return a + b;  // host builds of these helpers are compiled without contraction (tests) or see only rounded operands
+#endif
+}
+__host__ __device__ inline double fma_rn(double a, double b, double c) {
+#ifdef __CUDA_ARCH__
+  return __fma_rn(a, b, c);
+#else
+  return fma(a, b, c);
+#endif
+}
+
+// The free intrinsics columns of one PINHOLE / PINHOLE_RADIAL_TANGENTIAL observation from its normalised image point
+// (u, v) = q_xy / q_z and the group's intrinsics k, with the loss corrector P applied: Ji[j] = P00 c0 + P01 c1 and
+// Ji[NI + j] = P10 c0 + P11 c1 for the j-th column (c0, c1) of IMASK.  linearize_obs takes its J_i from here, and the passes over
+// a compact linearisation (kernels: kCompactIntr) rebuild J_i from the stored (u, v) with P = I, which is what the TRIVIAL loss
+// gives: every operation is rounded explicitly, so both produce the same bits.  The roundings are the ones nvcc chose for these
+// columns when linearize_obs computed them inline (r2 = u u + v v from two rounded products, 2 u u + r2 rounded on its own in
+// dk_9, the other sums fused), so J_i, and every solve, keeps the values it had before this helper existed.
+template <uint32_t IMASK>
+__host__ __device__ inline void obs_intr_cols(int model, double u, double v, const double* __restrict__ k, double P00, double P01,
+                                              double P10, double P11, double* Ji) {
+  constexpr int NI = popcount10(IMASK);
+  if (NI == 0) return;
+  const double f = k[0], ar = k[1], sk = k[2];
+  const double r2 = add_rn(mul_rn(u, u), mul_rn(v, v));
+  double ud, vd, dk[10][2];  // dk[j] = d(ud,vd)/dk_j, j >= 5
+  if (model == kModelPinhole) {
+    const double d = fma_rn(r2, fma_rn(k[6], r2, k[5]), 1.0);
+    ud = mul_rn(u, d); vd = mul_rn(v, d);
+    const double r4 = mul_rn(r2, r2);
+    dk[5][0] = mul_rn(r2, u); dk[5][1] = mul_rn(r2, v);
+    dk[6][0] = mul_rn(r4, u); dk[6][1] = mul_rn(r4, v);
+    dk[7][0] = dk[7][1] = dk[8][0] = dk[8][1] = dk[9][0] = dk[9][1] = 0.0;
+  } else {
+    const double r4 = mul_rn(r2, r2), r6 = mul_rn(r4, r2);
+    const double rd = fma_rn(mul_rn(k[7], r4), r2, fma_rn(k[6], r4, fma_rn(k[5], r2, 1.0)));
+    const double t1 = k[8], t2 = k[9];
+    const double uv2 = mul_rn(2.0 * u, v), eu = fma_rn(2.0 * u, u, r2), ev = fma_rn(2.0 * v, v, r2);
+    ud = fma_rn(mul_rn(2.0 * t1, u), v, fma_rn(u, rd, mul_rn(t2, eu)));
+    vd = fma_rn(mul_rn(2.0 * t2, u), v, fma_rn(v, rd, mul_rn(t1, ev)));
+    dk[5][0] = mul_rn(r2, u); dk[5][1] = mul_rn(r2, v);
+    dk[6][0] = mul_rn(r4, u); dk[6][1] = mul_rn(r4, v);
+    dk[7][0] = mul_rn(r6, u); dk[7][1] = mul_rn(r6, v);
+    dk[8][0] = uv2; dk[8][1] = ev;
+    dk[9][0] = add_rn(r2, mul_rn(2.0 * u, u)); dk[9][1] = uv2;
+  }
+  const double far = mul_rn(f, ar);
+  double col[10][2];
+  col[0][0] = ud;  col[0][1] = mul_rn(ar, vd);  // d/df
+  col[1][0] = 0.0; col[1][1] = mul_rn(f, vd);   // d/da
+  col[2][0] = vd;  col[2][1] = 0.0;             // d/ds
+  col[3][0] = 1.0; col[3][1] = 0.0;             // d/dcx
+  col[4][0] = 0.0; col[4][1] = 1.0;             // d/dcy
+  TBA_UNROLL
+  for (int j = 5; j < 10; ++j) {                // distortion params: K2 * d(ud,vd)/dk_j
+    col[j][0] = fma_rn(f, dk[j][0], mul_rn(sk, dk[j][1]));
+    col[j][1] = mul_rn(far, dk[j][1]);
+  }
+  TBA_UNROLL
+  for (int j = 0; j < NI; ++j) {
+    constexpr uint32_t M = IMASK;
+    const int idx = nth_bit(M, j);
+    Ji[j] = fma_rn(P00, col[idx][0], mul_rn(P01, col[idx][1]));
+    Ji[NI + j] = fma_rn(P10, col[idx][0], mul_rn(P11, col[idx][1]));
+  }
+}
+
 // Residual + analytic Jacobian + robust-loss correction (ceres Corrector).
 //   Ja[6] = rows of dpix/dX_{0..2}; Jw[6] = rows of dpix/dw; Jh[2]; Ji[2*NI] = row0 cols | row1 cols
 // of the stored intrinsics columns (bits of IMASK).  r[2] is the robustified residual,
-// rho0 the loss value (cost contribution 0.5 * rho0).
+// rho0 the loss value (cost contribution 0.5 * rho0); uv (optional) receives the normalised image point (u, v).
 template <uint32_t IMASK>
 __host__ __device__ inline bool linearize_obs(int model, const double* __restrict__ C, const double* __restrict__ rec,
                                      const double* __restrict__ k, const double X0, const double X1, const double X2,
                                      const double h, const double x, const double y, int loss_type, double loss_width,
-                                     double r[2], double& rho0, double Ja[6], double Jw[6], double Jh[2], double* Ji) {
+                                     double r[2], double& rho0, double Ja[6], double Jw[6], double Jh[2], double* Ji,
+                                     double* uv = nullptr) {
   constexpr int NI = popcount10(IMASK);
   const double* R = rec;
   const double* L = rec + 9;
@@ -195,17 +276,13 @@ __host__ __device__ inline bool linearize_obs(int model, const double* __restric
   const double iz = 1.0 / q2;
   const double u = q0 * iz, v = q1 * iz;
   const double r2 = u * u + v * v;
-  // distortion and its 2x2 derivative D' = d(ud,vd)/d(u,v); derivative columns w.r.t. distortion params
+  // distortion and its 2x2 derivative D' = d(ud,vd)/d(u,v)
   double ud, vd, D00, D01, D10, D11;
-  double dk[10][2];  // d(ud,vd)/d intr_j for j = 5.. ; only used entries are computed
   if (model == kModelPinhole) {
     const double d = 1.0 + r2 * (k[5] + k[6] * r2);
     const double dd = 2.0 * k[5] + 4.0 * k[6] * r2;
     ud = u * d; vd = v * d;
     D00 = d + u * u * dd; D01 = u * v * dd; D10 = D01; D11 = d + v * v * dd;
-    dk[5][0] = r2 * u; dk[5][1] = r2 * v;
-    dk[6][0] = r2 * r2 * u; dk[6][1] = r2 * r2 * v;
-    dk[7][0] = dk[7][1] = dk[8][0] = dk[8][1] = dk[9][0] = dk[9][1] = 0.0;
   } else {
     const double r4 = r2 * r2;
     const double rd = 1.0 + k[5] * r2 + k[6] * r4 + k[7] * r4 * r2;
@@ -217,11 +294,6 @@ __host__ __device__ inline bool linearize_obs(int model, const double* __restric
     D01 = 2.0 * u * v * rdp + 2.0 * t2 * v + 2.0 * t1 * u;
     D10 = 2.0 * u * v * rdp + 2.0 * t1 * u + 2.0 * t2 * v;
     D11 = rd + 2.0 * v * v * rdp + 6.0 * t1 * v + 2.0 * t2 * u;
-    dk[5][0] = r2 * u; dk[5][1] = r2 * v;
-    dk[6][0] = r4 * u; dk[6][1] = r4 * v;
-    dk[7][0] = r4 * r2 * u; dk[7][1] = r4 * r2 * v;
-    dk[8][0] = 2.0 * u * v; dk[8][1] = r2 + 2.0 * v * v;
-    dk[9][0] = r2 + 2.0 * u * u; dk[9][1] = 2.0 * u * v;
   }
   const double f = k[0], ar = k[1], sk = k[2];
   const double rr0 = f * ud + sk * vd + k[3] - x;
@@ -268,27 +340,8 @@ __host__ __device__ inline bool linearize_obs(int model, const double* __restric
   Jw[3] = -(c10 * L[0] + c11 * L[3] + c12 * L[6]);
   Jw[4] = -(c10 * L[1] + c11 * L[4] + c12 * L[7]);
   Jw[5] = -(c10 * L[2] + c11 * L[5] + c12 * L[8]);
-  // intrinsics columns (unrobustified), then P applied
-  if (NI > 0) {
-    double col[10][2];
-    col[0][0] = ud;  col[0][1] = ar * vd;   // d/df
-    col[1][0] = 0.0; col[1][1] = f * vd;    // d/da
-    col[2][0] = vd;  col[2][1] = 0.0;       // d/ds
-    col[3][0] = 1.0; col[3][1] = 0.0;       // d/dcx
-    col[4][0] = 0.0; col[4][1] = 1.0;       // d/dcy
-    TBA_UNROLL
-    for (int j = 5; j < 10; ++j) {          // distortion params: K2 * d(ud,vd)/dk_j
-      col[j][0] = f * dk[j][0] + sk * dk[j][1];
-      col[j][1] = f * ar * dk[j][1];
-    }
-    TBA_UNROLL
-    for (int j = 0; j < NI; ++j) {
-      constexpr uint32_t M = IMASK;
-      const int idx = nth_bit(M, j);
-      Ji[j] = P00 * col[idx][0] + P01 * col[idx][1];
-      Ji[NI + j] = P10 * col[idx][0] + P11 * col[idx][1];
-    }
-  }
+  obs_intr_cols<IMASK>(model, u, v, k, P00, P01, P10, P11, Ji);
+  if (uv) { uv[0] = u; uv[1] = v; }
   return true;
 }
 
@@ -405,11 +458,12 @@ template <uint32_t IMASK, bool EXT>
 __host__ __device__ inline bool linearize_obs_any(int model, const double* __restrict__ C, const double* __restrict__ rec,
                                                   const double* __restrict__ k, const double X0, const double X1, const double X2,
                                                   const double h, const double x, const double y, int loss_type, double loss_width,
-                                                  double r[2], double& rho0, double Ja[6], double Jw[6], double Jh[2], double* Ji) {
+                                                  double r[2], double& rho0, double Ja[6], double Jw[6], double Jh[2], double* Ji,
+                                                  double* uv = nullptr) {
   if (EXT) {
     if (model >= kModelFisheye) return linearize_obs_ext<IMASK>(model, C, rec, k, X0, X1, X2, h, x, y, loss_type, loss_width, r, rho0, Ja, Jw, Jh, Ji);
   }
-  return linearize_obs<IMASK>(model, C, rec, k, X0, X1, X2, h, x, y, loss_type, loss_width, r, rho0, Ja, Jw, Jh, Ji);
+  return linearize_obs<IMASK>(model, C, rec, k, X0, X1, X2, h, x, y, loss_type, loss_width, r, rho0, Ja, Jw, Jh, Ji, uv);
 }
 
 }  // namespace tba

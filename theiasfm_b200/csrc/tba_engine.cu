@@ -94,7 +94,7 @@ struct tba_context {
   std::string err;
   bool uploaded = false;
   tba_options opt;
-  uint32_t imask = 0;  // instantiated intrinsics column set
+  uint32_t imask = 0;  // instantiated intrinsics column set, | kCompactIntr for the compact layout of J
   int NI = 0, NJ = 14;
   DevProblem P;
   int n_cam = 0, n_group = 0, n_pt = 0, n_tiles = 0;
@@ -258,6 +258,10 @@ const uint32_t kMasks[] = {0x000u, 0x001u, 0x061u, 0x0E1u, 0x07Fu, 0x3FFu};
     case 0x061u: F(0x061u); break; \
     case 0x0E1u: F(0x0E1u); break; \
     case 0x07Fu: F(0x07Fu); break; \
+    case 0x061u | kCompactIntr: F(0x061u | kCompactIntr); break; \
+    case 0x0E1u | kCompactIntr: F(0x0E1u | kCompactIntr); break; \
+    case 0x07Fu | kCompactIntr: F(0x07Fu | kCompactIntr); break; \
+    case 0x3FFu | kCompactIntr: F(0x3FFu | kCompactIntr); break; \
     default: F(0x3FFu); break;  \
   }
 
@@ -1098,7 +1102,10 @@ int tba_upload(tba_context* c, const tba_options* options, const tba_problem* p)
   for (uint32_t m : kMasks) if ((H.union_free & ~m) == 0) { c->imask = m; break; }
   if (c->has_ext_models) c->imask = 0x3FFu;  // one instantiation for the other models: every intrinsics column stored
   c->NI = popcount10(c->imask);
-  c->NJ = 14 + 2 * c->NI;
+  // the compact layout of J (tba_kernels.cuh, kCompactIntr): the normalised image point (u, v) in place of the 2 NI doubles of J_i,
+  // which every pass over J rebuilds from it and the shared group's intrinsics
+  if (!c->has_ext_models && ng == 1 && options->loss_function_type == TBA_LOSS_TRIVIAL && c->NI >= 2) c->imask |= kCompactIntr;
+  c->NJ = nj_of(c->imask);
   const int npk = (int)H.pk2caller.size();
   const int n_long = H.n_long;
   const int n_tiles = H.n_tiles;
@@ -2074,10 +2081,26 @@ int tba_debug_linearize_raw(tba_context* c, int tile_kernel, int64_t* sizes_out,
   return TBA_OK;
 }
 
+int tba_debug_intr_cols(tba_context* c, int64_t* sizes_out, double* Ji) {
+  if (!c || !c->uploaded || !sizes_out) return TBA_ERR_INVALID_ARGUMENT;
+  CUDA_OK(c, cudaSetDevice(c->device));
+  sizes_out[0] = c->n_slots; sizes_out[1] = c->NI;
+  if (!Ji || c->NI == 0 || c->n_slots == 0) return TBA_OK;
+  DevBuf<double> d;
+  CUDA_OK(c, d.alloc((size_t)c->n_slots * 2 * c->NI));
+  const int grid = (int)((c->n_slots + 255) / 256);
+#define F(M) { auto kfn = k_debug_intr_cols<M>; LAUNCH(c, kfn, grid, 256, 0, c->P, (long long)c->n_slots, d.p); }
+  DISPATCH_IMASK(c->imask, F)
+#undef F
+  CUDA_OK(c, cudaMemcpyAsync(Ji, d.p, (size_t)c->n_slots * 2 * c->NI * 8, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_OK(c, cudaStreamSynchronize(c->stream));
+  return TBA_OK;
+}
+
 int tba_debug_stream_launch(tba_context* c, int32_t* out) {
   if (!c || !c->uploaded || !out) return TBA_ERR_INVALID_ARGUMENT;
   const int n_slices = c->n_normal_tiles * (TILE / 32);
-  out[0] = c->n_sm; out[1] = n_slices; out[2] = (int32_t)c->imask; out[3] = c->has_ext_models ? 1 : 0;
+  out[0] = c->n_sm; out[1] = n_slices; out[2] = (int32_t)(c->imask & ~kCompactIntr); out[3] = c->has_ext_models ? 1 : 0;
   auto put = [&](int k, int NW, int NS) { out[4 + 3 * k] = stream_grid(c, n_slices, NW); out[5 + 3 * k] = NW; out[6 + 3 * k] = NS; };
 #define F(M) { put(0, LinCfg<M>::NW, LinCfg<M>::NS); put(1, PrepCfg<M>::NW, PrepCfg<M>::NS); \
                put(2, StreamCfg<M, 0>::NW, StreamCfg<M, 0>::NS); put(3, StreamCfg<M, 1>::NW, StreamCfg<M, 1>::NS); }

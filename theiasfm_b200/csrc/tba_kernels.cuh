@@ -23,6 +23,15 @@ constexpr int MAXP = 256;   // max points per tile
 constexpr int VB = 64;      // CTAs of the camera-space vector kernels (deterministic reductions)
 constexpr int VT = 256;
 
+// Layout of the stored linearisation, rows of NJ doubles per observation: J_a (6) | J_w (6) | J_h (2), then either the NI free
+// intrinsics columns J_i (2 NI), or, in the COMPACT layout (kCompactIntr set in IMASK), the normalised image point (u, v), from which
+// every pass over J rebuilds J_i (obs_rebuild_Ji).  The engine selects the compact layout when it stores fewer bytes (NI >= 2) and
+// J_i is a function of (u, v) and uniform values alone: PINHOLE / PINHOLE_RADIAL_TANGENTIAL, one shared intrinsics group and the
+// TRIVIAL loss (the corrector is the identity).
+constexpr uint32_t kCompactIntr = 1u << 16;  // outside the ten intrinsics bits: popcount10 and nth_bit do not see it
+__host__ __device__ constexpr bool compact_intr(uint32_t imask) { return (imask & kCompactIntr) != 0; }
+__host__ __device__ constexpr int nj_of(uint32_t imask) { return compact_intr(imask) ? 16 : 14 + 2 * popcount10(imask); }
+
 // Device view of the packed problem.
 struct DevProblem {
   int n_cam, n_group, n_pt, n_tiles;
@@ -48,7 +57,7 @@ struct DevProblem {
   const int* tile_nruns;       // [n_tiles]
   const uint8_t* tile_flags;   // [n_tiles] bit0: long tile (tracks > 32 observations; points may straddle warps)
   const double* xy;            // [tile][2][TILE]
-  double* J;                   // [tile][NJ][TILE], NJ = 14 + 2 NI
+  double* J;                   // [tile][NJ][TILE], NJ = nj_of(IMASK)
   double* res;                 // [tile][2][TILE] robustified residuals
   // per point
   double* Hpp;                 // [n_pt][10] sym J_p^T J_p (unscaled)
@@ -198,14 +207,14 @@ __device__ __forceinline__ void sym4_mul(const double* __restrict__ M, const dou
 // change to an expression here changes both.  A row set is a pointer plus a compile-time element stride: 32 for a warp's
 // shared-memory stage ([row][32 lanes]), 1 for a register array.  SP: stride of J_a and J_h; SC: stride of J_w and J_i.
 
-// w = F x = J_c x_c + J_i x_i
-template <int NI, int SP, int SC>
+// w = F x = J_c x_c + J_i x_i  (SI: stride of J_i)
+template <int NI, int SP, int SC, int SI = SC>
 __device__ __forceinline__ void obs_apply_F(const double* ja, const double* jw, const double* ji, double h, double2 xa, double2 xb,
                                             double2 xc, const double* xi, double& w0, double& w1) {
   w0 = -h * (ja[0] * xa.x + ja[SP] * xa.y + ja[2 * SP] * xb.x) + jw[0] * xb.y + jw[SC] * xc.x + jw[2 * SC] * xc.y;
   w1 = -h * (ja[3 * SP] * xa.x + ja[4 * SP] * xa.y + ja[5 * SP] * xb.x) + jw[3 * SC] * xb.y + jw[4 * SC] * xc.x + jw[5 * SC] * xc.y;
 #pragma unroll
-  for (int j = 0; j < NI; ++j) { w0 += ji[j * SC] * xi[j]; w1 += ji[(NI + j) * SC] * xi[j]; }
+  for (int j = 0; j < NI; ++j) { w0 += ji[j * SI] * xi[j]; w1 += ji[(NI + j) * SI] * xi[j]; }
 }
 // t = J_p^T w
 template <int SP>
@@ -293,9 +302,10 @@ __device__ __forceinline__ int tri10(int ia, int ib) { return ia * 10 - ia * (ia
 
 // Linearisation: Ceres' bookkeeping of one observation.  A failed projection counts as a failure; one whose parameter blocks
 // are all constant goes to the fixed cost (Ceres removes the residual: fixed_cost).  Either way its rows and residual are zeroed.
+// uv: the normalised image point, set to NaN when the rows are zeroed (the mark obs_rebuild_Ji reads).
 template <int NI>
 __device__ __forceinline__ void obs_settle(bool ok, bool is_fixed, double rho0, double& cost, double& fixed, double& failed, double Ja[6],
-                                           double Jw[6], double Jh[2], double Ji[], double r[2]) {
+                                           double Jw[6], double Jh[2], double Ji[], double uv[2], double r[2]) {
   if (!ok) failed += 1.0;
   else if (is_fixed) fixed += 0.5 * rho0;
   else cost += 0.5 * rho0;
@@ -305,20 +315,28 @@ __device__ __forceinline__ void obs_settle(bool ok, bool is_fixed, double rho0, 
     Jh[0] = Jh[1] = 0.0; r[0] = r[1] = 0.0;
 #pragma unroll
     for (int j = 0; j < 2 * NI; ++j) Ji[j] = 0.0;
+    uv[0] = uv[1] = nan("");
   }
 }
-// Stores the observation's compact rows into its warp slice (Jt, rt: the lane's element of row 0; [NJ][32] and [2][32]).
-template <int NI>
+// Stores the observation's rows into its warp slice (Jt, rt: the lane's element of row 0; [NJ][32] and [2][32]): J_i, or (u, v)
+// in the compact layout.
+template <uint32_t IMASK>
 __device__ __forceinline__ void obs_store(double* Jt, double* rt, const double Ja[6], const double Jw[6], const double Jh[2], const double Ji[],
-                                          const double r[2]) {
+                                          const double uv[2], const double r[2]) {
+  constexpr int NI = popcount10(IMASK);
 #pragma unroll
   for (int j = 0; j < 6; ++j) Jt[j * 32] = Ja[j];
 #pragma unroll
   for (int j = 0; j < 6; ++j) Jt[(6 + j) * 32] = Jw[j];
   Jt[12 * 32] = Jh[0];
   Jt[13 * 32] = Jh[1];
+  if (compact_intr(IMASK)) {
+    Jt[14 * 32] = uv[0];
+    Jt[15 * 32] = uv[1];
+  } else {
 #pragma unroll
-  for (int j = 0; j < 2 * NI; ++j) Jt[(14 + j) * 32] = Ji[j];
+    for (int j = 0; j < 2 * NI; ++j) Jt[(14 + j) * 32] = Ji[j];
+  }
   rt[0] = r[0];
   rt[32] = r[1];
 }
@@ -351,6 +369,19 @@ __device__ __forceinline__ void obs_intr_grad(const double Ji[], const double r[
   cn = Ji[j] * Ji[j] + Ji[NI + j] * Ji[NI + j];
 }
 
+// J_i of one observation of a compact linearisation from its stored (u, v) and the shared group's model and intrinsics k: the same
+// bits linearize_obs returned (the corrector of the TRIVIAL loss is exactly the identity).  A NaN u marks an observation whose rows
+// were zeroed (padding, failed projection, constant parameter blocks): its J_i is zero.  The streaming kernels read k from a
+// per-warp copy in shared memory (kept in registers across their loops, the ten doubles make them spill).
+template <uint32_t IMASK>
+__device__ __forceinline__ void obs_rebuild_Ji(int model, const double* k, double u, double v, double Ji[]) {
+  constexpr int NI = popcount10(IMASK);
+  obs_intr_cols<IMASK>(model, u, v, k, 1.0, 0.0, 0.0, 1.0, Ji);
+  const bool live = u == u;
+#pragma unroll
+  for (int j = 0; j < 2 * NI; ++j) Ji[j] = live ? Ji[j] : 0.0;
+}
+
 // ---------------------------------------------------------- K1 linearise
 // One thread per observation slot.  Writes the compact linearisation and the robustified residual
 // ([tile][warp][NJ][32] / [tile][warp][2][32]: a warp's slice is contiguous), the per-point blocks, the camera-side
@@ -367,7 +398,7 @@ __global__ void __launch_bounds__(TILE, EXT ? 1 : 3) k_linearize(DevProblem P, d
                                                            double* __restrict__ rep, int tile0) {
   constexpr bool STAGED_RED = !EXT;
   constexpr int NI = popcount10(IMASK);
-  constexpr int NJ = 14 + 2 * NI;
+  constexpr int NJ = nj_of(IMASK);
   __shared__ double s_acc[MAXP][14];
   const int tile = tile0 + blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const bool long_tile = (P.tile_flags[tile] & 1) != 0;
@@ -381,7 +412,7 @@ __global__ void __launch_bounds__(TILE, EXT ? 1 : 3) k_linearize(DevProblem P, d
   const bool valid = cam >= 0;
   double cost = 0.0, fixed = 0.0, failed = 0.0;
   double Ja[6] = {0, 0, 0, 0, 0, 0}, Jw[6] = {0, 0, 0, 0, 0, 0}, Jh[2] = {0, 0}, r[2] = {0, 0};
-  double Ji[2 * NI + 1];
+  double Ji[2 * NI + 1], uv[2] = {nan(""), nan("")};
 #pragma unroll
   for (int j = 0; j < 2 * NI; ++j) Ji[j] = 0.0;
   int pl = -1 - lane, grp = 0;  // padding lanes: unique negative keys (each its own run)
@@ -399,11 +430,11 @@ __global__ void __launch_bounds__(TILE, EXT ? 1 : 3) k_linearize(DevProblem P, d
     gather_camera(P.ext, P.cam_s4, cam, Cw, rec);
     const bool ok = linearize_obs_any<IMASK, EXT>(P.group_model[grp], Cw, rec,
                                          P.intr + (size_t)grp * 10, X.x, X.y, X.z, X.w, x, y, P.loss_type, P.loss_width,
-                                         r, rho0, Ja, Jw, Jh, Ji);
-    obs_settle<NI>(ok, (P.slot_flags[slot] & 1) != 0, rho0, cost, fixed, failed, Ja, Jw, Jh, Ji, r);
+                                         r, rho0, Ja, Jw, Jh, Ji, uv);
+    obs_settle<NI>(ok, (P.slot_flags[slot] & 1) != 0, rho0, cost, fixed, failed, Ja, Jw, Jh, Ji, uv, r);
   }
   // store the compact linearisation (each warp writes 256-byte rows of its own slice)
-  obs_store<NI>(P.J + wslice(tile, warp, NJ) + lane, P.res + wslice(tile, warp, 2) + lane, Ja, Jw, Jh, Ji, r);
+  obs_store<IMASK>(P.J + wslice(tile, warp, NJ) + lane, P.res + wslice(tile, warp, 2) + lane, Ja, Jw, Jh, Ji, uv, r);
   // per-point blocks H_pp, g_p
   {
     double acc[14];
@@ -792,10 +823,11 @@ __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.p
 // emitted element-major (warp_red_rows); intrinsics sums: warp reduce + RED to a replica row (one shared group) or one RED
 // per lane.  Correct for any tile.  Dynamic shared memory: TILE * (NJ + 2) doubles.
 template <uint32_t IMASK, int MODE>
-__global__ void __launch_bounds__(TILE, (14 + 2 * popcount10(IMASK)) <= 20 ? 4 : 2) k_schur(DevProblem P, const double* __restrict__ xs, double* __restrict__ y,
+__global__ void __launch_bounds__(TILE, popcount10(IMASK) <= 3 ? 4 : 2) k_schur(DevProblem P, const double* __restrict__ xs, double* __restrict__ y,
                                                 double* __restrict__ rep, const int* __restrict__ done_flag, int tile0) {
   constexpr int NI = popcount10(IMASK);
-  constexpr int NJ = 14 + 2 * NI;
+  constexpr int NJ = nj_of(IMASK);
+  constexpr bool CI = compact_intr(IMASK);
   constexpr int WS = (NJ + 2) * 32;  // doubles per warp stage
   if (done_flag != nullptr && *done_flag) return;
 #ifdef TBA_EMULATE
@@ -842,12 +874,15 @@ __global__ void __launch_bounds__(TILE, (14 + 2 * popcount10(IMASK)) <= 20 ? 4 :
   const bool head = lane == 0 || prev != pl;
   __syncthreads();  // s_t zeroed
   mbar_wait(&s_bar[warp], 0);  // this warp's slice landed in shared memory
-  // the lane's rows in the stage (stride 32)
-  const double *ja = sJ + lane, *jw = ja + 6 * 32, *jh = ja + 12 * 32, *ji = ja + 14 * 32;
+  // the lane's rows in the stage (stride 32); J_i in registers when rebuilt from (u, v)
+  constexpr int SI = CI ? 1 : 32;
+  double jir[2 * NI + 1];
+  if (CI) obs_rebuild_Ji<IMASK>(P.group_model[0], P.intr, sJ[14 * 32 + lane], sJ[15 * 32 + lane], jir);
+  const double *ja = sJ + lane, *jw = ja + 6 * 32, *jh = ja + 12 * 32, *ji = CI ? jir : ja + 14 * 32;
   double w0 = 0.0, w1 = 0.0, r0 = 0.0, r1 = 0.0;
   if (valid) {
     if (MODE != 0) { r0 = sR[lane]; r1 = sR[32 + lane]; }
-    if (MODE != 1) obs_apply_F<NI, 32, 32>(ja, jw, ji, h, xa, xb, xc, xi, w0, w1);
+    if (MODE != 1) obs_apply_F<NI, 32, 32, SI>(ja, jw, ji, h, xa, xb, xc, xi, w0, w1);
     if (MODE == 1) { w0 = r0; w1 = r1; }
     if (MODE == 2) { w0 = r0 - w0; w1 = r1 - w1; }
   }
@@ -886,7 +921,7 @@ __global__ void __launch_bounds__(TILE, (14 + 2 * popcount10(IMASK)) <= 20 ? 4 :
     // camera-side contributions staged per warp and emitted element-major (warp_red_rows)
     double yv[6], yi[NI + 1];
     obs_JcT<32, 32>(ja, jw, h, z0, z1, yv);
-    obs_JiT<NI, 32>(ji, z0, z1, yi);
+    obs_JiT<NI, SI>(ji, z0, z1, yi);
 #pragma unroll
     for (int j = 0; j < 6; ++j) yv[j] = valid ? yv[j] : 0.0;
 #pragma unroll
@@ -1006,13 +1041,15 @@ __device__ __forceinline__ void warp_red_rows_cols(double* __restrict__ dst, con
 template <uint32_t IMASK, int MODE>
 struct StreamCfg {
   static constexpr int NI = popcount10(IMASK);
-  static constexpr int NJ = 14 + 2 * NI;
+  static constexpr int NJ = nj_of(IMASK);
   static constexpr int STG = NJ * 32 + (MODE != 0 ? 64 : 0) + 32;  // doubles per stage: J | [res] | cam ids (32 int) + point ids (32 int)
   static constexpr int NS = 3;                                      // ring depth
   // warps per CTA: what fits 220 KB of dynamic shared memory with NS stages, at most 12 (384 threads leave 168 registers per
-  // thread: the software-pipelined gathers of the next slice live in registers next to the current slice's)
-  static constexpr int NW = (220 * 1024 / (NS * STG * 8)) > 12 ? 12 : (220 * 1024 / (NS * STG * 8));
-  static constexpr size_t SMEM = (size_t)NW * NS * STG * 8 + (size_t)NW * NS * 8;
+  // thread: the software-pipelined gathers of the next slice live in registers next to the current slice's); the J_i rebuild of
+  // the compact layout with NI > 3 needs 255 registers: at most 8
+  static constexpr int NWMAX = compact_intr(IMASK) && NI > 3 ? 8 : 12;
+  static constexpr int NW = (220 * 1024 / (NS * STG * 8)) > NWMAX ? NWMAX : (220 * 1024 / (NS * STG * 8));
+  static constexpr size_t SMEM = (size_t)NW * NS * STG * 8 + (size_t)NW * NS * 8 + (compact_intr(IMASK) ? (size_t)NW * 10 * 8 : 0);
 };
 
 template <uint32_t IMASK, int MODE>
@@ -1021,6 +1058,7 @@ k_schur_stream(DevProblem P, const double* __restrict__ xs, double* __restrict__
                const int* __restrict__ done_flag, int n_slices, P2pDev pp) {
   using Cfg = StreamCfg<IMASK, MODE>;
   constexpr int NI = Cfg::NI, NJ = Cfg::NJ, STG = Cfg::STG, NS = Cfg::NS, NW = Cfg::NW;
+  constexpr bool CI = compact_intr(IMASK);  // (implies one shared group)
   if (done_flag != nullptr && *done_flag) return;
 #ifdef TBA_EMULATE
   double* s_dyn = emu::dyn_smem<double>();
@@ -1033,6 +1071,7 @@ k_schur_stream(DevProblem P, const double* __restrict__ xs, double* __restrict__
   const bool active = s_begin < s_end;  // warp-uniform; idle warps fall through to the end (the multi-GPU epilogue has block barriers)
   double* ring = s_dyn + (size_t)warp * NS * STG;
   uint64_t* bars = reinterpret_cast<uint64_t*>(s_dyn + (size_t)NW * NS * STG) + warp * NS;
+  double* s_k = s_dyn + (size_t)NW * NS * STG + (size_t)NW * NS + warp * 10;  // CI: the warp's copy of the group's intrinsics
   constexpr uint32_t jbytes = NJ * 32 * 8, rbytes = (MODE != 0) ? 2 * 32 * 8 : 0;
   auto issue = [&](int stage, int slice) {  // lane 0 only
     double* st = ring + (size_t)stage * STG;
@@ -1050,7 +1089,10 @@ k_schur_stream(DevProblem P, const double* __restrict__ xs, double* __restrict__
     for (int k = 0; k < NS; ++k) if (s_begin + k < s_end) issue(k, s_begin + k);
   }
   __syncwarp();
-  // intrinsics x of the single shared group: one uniform load for the whole kernel
+  // intrinsics x of the single shared group: one uniform load for the whole kernel; its model and intrinsics for the J_i rebuild
+  const int model0 = CI ? P.group_model[0] : 0;
+  if (CI && lane < 10) s_k[lane] = P.intr[lane];
+  __syncwarp();
   double xi_u[NI + 1];
   if (NI > 0 && MODE != 1 && P.single_group) {
 #pragma unroll
@@ -1117,8 +1159,12 @@ k_schur_stream(DevProblem P, const double* __restrict__ xs, double* __restrict__
     const int stage = it % NS;
     double* sJ = ring + (size_t)stage * STG;
     const double* sR = sJ + NJ * 32;
-    // J_a and J_h of this lane in registers (every element read from shared memory exactly once), J_w and J_i in the stage
-    const double *jw = sJ + lane + 6 * 32, *ji = sJ + lane + 14 * 32;
+    // J_a and J_h of this lane in registers (every element read from shared memory exactly once), J_w in the stage; J_i in the
+    // stage, or rebuilt in registers from (u, v)
+    constexpr int SI = CI ? 1 : 32;
+    double jir[2 * NI + 1];
+    if (CI) obs_rebuild_Ji<IMASK>(model0, s_k, sJ[14 * 32 + lane], sJ[15 * 32 + lane], jir);
+    const double *jw = sJ + lane + 6 * 32, *ji = CI ? jir : sJ + lane + 14 * 32;
     double w0 = 0.0, w1 = 0.0, r0 = 0.0, r1 = 0.0;
     double ja[6], jh[2];
 #pragma unroll
@@ -1126,7 +1172,7 @@ k_schur_stream(DevProblem P, const double* __restrict__ xs, double* __restrict__
     jh[0] = sJ[12 * 32 + lane]; jh[1] = sJ[13 * 32 + lane];
     if (valid) {
       if (MODE != 0) { r0 = sR[lane]; r1 = sR[32 + lane]; }
-      if (MODE != 1) obs_apply_F<NI, 1, 32>(ja, jw, ji, h, xa, xb, xc, xi, w0, w1);
+      if (MODE != 1) obs_apply_F<NI, 1, 32, SI>(ja, jw, ji, h, xa, xb, xc, xi, w0, w1);
       if (MODE == 1) { w0 = r0; w1 = r1; }
       if (MODE == 2) { w0 = r0 - w0; w1 = r1 - w1; }
     }
@@ -1158,7 +1204,7 @@ k_schur_stream(DevProblem P, const double* __restrict__ xs, double* __restrict__
     } else {
       double yv[6], yi[NI + 1];
       obs_JcT<1, 32>(ja, jw, h, z0, z1, yv);
-      obs_JiT<NI, 32>(ji, z0, z1, yi);
+      obs_JiT<NI, SI>(ji, z0, z1, yi);
 #pragma unroll
       for (int j = 0; j < 6; ++j) yv[j] = valid ? yv[j] : 0.0;
 #pragma unroll
@@ -1169,12 +1215,12 @@ k_schur_stream(DevProblem P, const double* __restrict__ xs, double* __restrict__
       __syncwarp();
       if (!(MODE == 0 && (P.ablate & 1))) warp_red_rows<6>(y, sJ, sbase, lane);
       if (NI > 0) {
-        if (P.single_group) {
+        if (CI || P.single_group) {
 #pragma unroll
           for (int j = 0; j < NI; ++j) yi_acc[j] += yi[j];
         } else {
           // per-group intrinsics rows: staged behind the extrinsics rows ([32][NI] doubles + 32 ints) and emitted element-major
-          static_assert(32 * 6 + 16 + 32 * NI + 16 <= NJ * 32, "stage too small for the intrinsics staging");
+          static_assert(CI || 32 * 6 + 16 + 32 * NI + 16 <= NJ * 32, "stage too small for the intrinsics staging");
           double* si = sJ + 32 * 6 + 16;
           int* sibase = reinterpret_cast<int*>(si + 32 * NI);
           __syncwarp();
@@ -1264,13 +1310,15 @@ k_schur_stream(DevProblem P, const double* __restrict__ xs, double* __restrict__
 template <uint32_t IMASK>
 struct PrepCfg {
   static constexpr int NI = popcount10(IMASK);
-  static constexpr int NJ = 14 + 2 * NI;
+  static constexpr int NJ = nj_of(IMASK);
   static constexpr int NSI = NI * (NI + 1) / 2;
   static constexpr int STG = NJ * 32 + 64 + 32;
   static constexpr int NS = 3;
-  static constexpr int NWMAX = NI <= 4 ? 10 : 6;  // register budget: NI <= 4: 192 registers per thread, else 255
+  // register budget: NI <= 4 (NI <= 3 with the J_i rebuild of the compact layout): 192 registers per thread, else 255
+  static constexpr int NWMAX = NI <= (compact_intr(IMASK) ? 3 : 4) ? 10 : 6;
   static constexpr int NW = (216 * 1024 / (NS * STG * 8)) > NWMAX ? NWMAX : (216 * 1024 / (NS * STG * 8));
-  static constexpr size_t SMEM = (size_t)NW * NS * STG * 8 + (size_t)NW * NS * 8 + (size_t)NW * (NSI + 1) * 8;
+  static constexpr size_t SMEM = (size_t)NW * NS * STG * 8 + (size_t)NW * NS * 8 + (size_t)NW * (NSI + 1) * 8 +
+                                 (compact_intr(IMASK) ? (size_t)NW * 10 * 8 : 0);
 };
 
 template <uint32_t IMASK>
@@ -1278,6 +1326,7 @@ __global__ void __launch_bounds__(PrepCfg<IMASK>::NW * 32, 1)
 k_prepare_stream(DevProblem P, double* __restrict__ y, double* __restrict__ Sc, double* __restrict__ Si, double* __restrict__ rep, int n_slices) {
   using Cfg = PrepCfg<IMASK>;
   constexpr int NI = Cfg::NI, NJ = Cfg::NJ, STG = Cfg::STG, NS = Cfg::NS, NW = Cfg::NW, NSI = Cfg::NSI;
+  constexpr bool CI = compact_intr(IMASK);  // (implies one shared group)
 #ifdef TBA_EMULATE
   double* s_dyn = emu::dyn_smem<double>();
 #else
@@ -1289,6 +1338,7 @@ k_prepare_stream(DevProblem P, double* __restrict__ y, double* __restrict__ Sc, 
   double* ring = s_dyn + (size_t)warp * NS * STG;
   uint64_t* bars = reinterpret_cast<uint64_t*>(s_dyn + (size_t)NW * NS * STG) + warp * NS;
   double* s_si = s_dyn + (size_t)NW * NS * STG + (size_t)NW * NS;  // [NW][NSI + 1] end-of-kernel partials of the shared-group block
+  double* s_k = s_si + (size_t)NW * (NSI + 1) + warp * 10;          // CI: the warp's copy of the group's intrinsics
   constexpr uint32_t jbytes = NJ * 32 * 8, rbytes = 2 * 32 * 8;
   auto issue = [&](int stage, int slice) {  // lane 0 only
     double* st = ring + (size_t)stage * STG;
@@ -1305,6 +1355,9 @@ k_prepare_stream(DevProblem P, double* __restrict__ y, double* __restrict__ Sc, 
 #pragma unroll
     for (int k = 0; k < NS; ++k) if (s_begin + k < s_end) issue(k, s_begin + k);
   }
+  __syncwarp();
+  const int model0 = CI ? P.group_model[0] : 0;
+  if (CI && lane < 10) s_k[lane] = P.intr[lane];
   __syncwarp();
   double yi_acc[NI + 1], si_acc[NSI + 1];
 #pragma unroll
@@ -1353,8 +1406,12 @@ k_prepare_stream(DevProblem P, double* __restrict__ y, double* __restrict__ Sc, 
 #pragma unroll
     for (int j = 0; j < 6; ++j) { ja[j] = Jt[j * 32]; jw[j] = Jt[(6 + j) * 32]; }
     jh[0] = Jt[12 * 32]; jh[1] = Jt[13 * 32];
+    if (CI) {
+      obs_rebuild_Ji<IMASK>(model0, s_k, Jt[14 * 32], Jt[15 * 32], ji);
+    } else {
 #pragma unroll
-    for (int j = 0; j < 2 * NI; ++j) ji[j] = Jt[(14 + j) * 32];
+      for (int j = 0; j < 2 * NI; ++j) ji[j] = Jt[(14 + j) * 32];
+    }
     double r0 = 0.0, r1 = 0.0;
     if (valid) { r0 = sR[lane]; r1 = sR[32 + lane]; }
     if (!valid) {
@@ -1488,7 +1545,7 @@ k_prepare_stream(DevProblem P, double* __restrict__ y, double* __restrict__ Sc, 
 template <uint32_t IMASK>
 struct LinCfg {
   static constexpr int NI = popcount10(IMASK);
-  static constexpr int NJ = 14 + 2 * NI;
+  static constexpr int NJ = nj_of(IMASK);
   static constexpr int STG = 64 + 16 + 16 + 4;  // doubles per stage: xy [2][32] | cam ids (32 int) | point ids (32 int) | flags (32 bytes)
   static constexpr int RSTG = 2 * 32 * 6 + 16;  // camera-row staging per warp: gradient [32][6] | column norms [32][6] | 32 ints
   static constexpr int NS = 4;                  // ring depth
@@ -1571,7 +1628,7 @@ k_linearize_stream(DevProblem P, double* __restrict__ g_cs, double* __restrict__
     const int stage = it % NS;
     const double* st = ring + (size_t)stage * STG;
     double Ja[6] = {0, 0, 0, 0, 0, 0}, Jw[6] = {0, 0, 0, 0, 0, 0}, Jh[2] = {0, 0}, r[2] = {0, 0};
-    double Ji[2 * NI + 1];
+    double Ji[2 * NI + 1], uv[2] = {nan(""), nan("")};
 #pragma unroll
     for (int j = 0; j < 2 * NI; ++j) Ji[j] = 0.0;
     if (valid) {
@@ -1591,11 +1648,11 @@ k_linearize_stream(DevProblem P, double* __restrict__ g_cs, double* __restrict__
 #endif
       double rho0 = 0.0;
       const bool ok = linearize_obs_any<IMASK, false>(P.group_model[grp], Cw, rec, P.intr + (size_t)grp * 10, X01.x, X01.y, X23.x,
-                                                      X23.y, st[lane], st[32 + lane], P.loss_type, P.loss_width, r, rho0, Ja, Jw, Jh, Ji);
+                                                      X23.y, st[lane], st[32 + lane], P.loss_type, P.loss_width, r, rho0, Ja, Jw, Jh, Ji, uv);
       obs_settle<NI>(ok, (reinterpret_cast<const uint8_t*>(st + 96)[lane] & 1) != 0, rho0, cost_acc, fixed_acc, failed_acc, Ja, Jw, Jh,
-                     Ji, r);
+                     Ji, uv, r);
     }
-    obs_store<NI>(P.J + (size_t)s * NJ * 32 + lane, P.res + (size_t)s * 64 + lane, Ja, Jw, Jh, Ji, r);
+    obs_store<IMASK>(P.J + (size_t)s * NJ * 32 + lane, P.res + (size_t)s * 64 + lane, Ja, Jw, Jh, Ji, uv, r);
     // per-point blocks H_pp, g_p
     {
       double acc[14];
@@ -1673,8 +1730,7 @@ k_linearize_stream(DevProblem P, double* __restrict__ g_cs, double* __restrict__
 // The 21 block entries of every observation are staged per warp and emitted element-major (warp_red_rows).
 template <uint32_t IMASK>
 __global__ void __launch_bounds__(TILE) k_precond_ext(DevProblem P, double* __restrict__ Sc, int tile0) {
-  constexpr int NI = popcount10(IMASK);
-  constexpr int NJ = 14 + 2 * NI;
+  constexpr int NJ = nj_of(IMASK);
   const int tile = tile0 + blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const size_t slot = (size_t)tile * TILE + tid;
   const int cam = P.slot_cam[slot];
@@ -1705,7 +1761,7 @@ __global__ void __launch_bounds__(TILE) k_precond_ext(DevProblem P, double* __re
 template <uint32_t IMASK>
 __global__ void __launch_bounds__(TILE) k_precond_intr(DevProblem P, double* __restrict__ Si, int tile0) {
   constexpr int NI = popcount10(IMASK);
-  constexpr int NJ = 14 + 2 * NI;
+  constexpr int NJ = nj_of(IMASK);
   constexpr int NW = 4 * NI;
   constexpr int NS = NI * (NI + 1) / 2;
 #ifdef TBA_EMULATE
@@ -1734,8 +1790,12 @@ __global__ void __launch_bounds__(TILE) k_precond_intr(DevProblem P, double* __r
     for (int j = 0; j < 3; ++j) { jp0[j] = Jt[j * 32]; jp1[j] = Jt[(3 + j) * 32]; }
     jp0[3] = Jt[12 * 32];
     jp1[3] = Jt[13 * 32];
+    if (compact_intr(IMASK)) {
+      obs_rebuild_Ji<IMASK>(P.group_model[0], P.intr, Jt[14 * 32], Jt[15 * 32], Ji);
+    } else {
 #pragma unroll
-    for (int j = 0; j < 2 * NI; ++j) Ji[j] = Jt[(14 + j) * 32];
+      for (int j = 0; j < 2 * NI; ++j) Ji[j] = Jt[(14 + j) * 32];
+    }
     grp = P.cam_group[cam];
     const int run = P.slot_run[slot];
     if (run >= 0) {
@@ -1776,6 +1836,27 @@ __global__ void __launch_bounds__(TILE) k_precond_intr(DevProblem P, double* __r
       }
       ++n;
     }
+}
+
+// Debug read-back: the J_i of every slot as the passes over J see it, out [n_slots / 32][2 NI][32] (the rows 14.. of the full
+// layout): rebuilt from the stored (u, v) in the compact layout, copied otherwise.
+template <uint32_t IMASK>
+__global__ void k_debug_intr_cols(DevProblem P, long long n_slots, double* __restrict__ out) {
+  constexpr int NI = popcount10(IMASK), NJ = nj_of(IMASK);
+  const long long s = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= n_slots) return;
+  const long long slice = s >> 5;
+  const int lane = (int)(s & 31);
+  const double* Jt = P.J + (size_t)slice * NJ * 32 + lane;
+  double Ji[2 * NI + 1];
+  if (compact_intr(IMASK)) {
+    obs_rebuild_Ji<IMASK>(P.group_model[0], P.intr, Jt[14 * 32], Jt[15 * 32], Ji);
+  } else {
+#pragma unroll
+    for (int j = 0; j < 2 * NI; ++j) Ji[j] = Jt[(14 + j) * 32];
+  }
+#pragma unroll
+  for (int j = 0; j < 2 * NI; ++j) out[((size_t)slice * 2 * NI + j) * 32 + lane] = Ji[j];
 }
 
 // In-place Cholesky inverse of an n x n SPD matrix held in registers/local (row-major, n <= 10).

@@ -20,7 +20,7 @@ _LIB = None
 EXPORTED_SYMBOLS = [
     "tba_options_init", "tba_device_count", "tba_create", "tba_destroy", "tba_nccl_unique_id", "tba_last_error",
     "tba_solve", "tba_upload", "tba_minimize", "tba_download", "tba_shard_points", "tba_debug_linearize", "tba_debug_linearize_raw",
-    "tba_debug_stream_launch",
+    "tba_debug_stream_launch", "tba_debug_intr_cols",
     "tba_debug_prepare_linear_system", "tba_debug_schur_matvec", "tba_debug_solve_linear_system",
     "tba_debug_evaluate_step", "tba_debug_read", "tba_reset_parameters", "tba_set_max_iterations", "tba_set_profiling", "tba_get_profile", "tba_get_profile_stages", "tba_solve_multi", "tba_debug_pack", "tba_filter_tracks", "tba_adjust_tracks", "tba_adjust_views", "tba_estimate_tracks", "tba_two_view_ba_batch", "tba_two_view_ba_batch_multi",
 ]
@@ -55,6 +55,7 @@ def lib():
         L.tba_debug_linearize.argtypes = [C.c_void_p, dp]
         L.tba_debug_linearize_raw.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_int64), dp, dp, dp, dp, dp]
         L.tba_debug_stream_launch.argtypes = [C.c_void_p, C.POINTER(C.c_int32)]
+        L.tba_debug_intr_cols.argtypes = [C.c_void_p, C.POINTER(C.c_int64), dp]
         L.tba_debug_prepare_linear_system.argtypes = [C.c_void_p, C.c_double]
         L.tba_debug_schur_matvec.argtypes = [C.c_void_p, dp, dp, dp, dp]
         L.tba_debug_solve_linear_system.argtypes = [C.c_void_p, C.POINTER(C.c_int32), dp]
@@ -343,6 +344,16 @@ class Engine:
                                                   _dp(J), _dp(res), _dp(Hpp), _dp(gp), _dp(lin)))
         return dict(J=J, res=res, Hpp=Hpp, gp=gp, g=lin[:ncs], cn=lin[ncs:2 * ncs], cost=lin[2 * ncs], fixed=lin[2 * ncs + 1],
                     failed=lin[2 * ncs + 2])
+
+    def intr_cols_raw(self):
+        """tba_debug_intr_cols: J_i [slices, 2 NI, 32] of the last linearisation as the passes over J see it (rebuilt from the stored
+        normalised image point in the compact layout), in the order of linearize_raw()["J"][:, 14:] in the full layout."""
+        sizes = np.zeros(2, np.int64)
+        self._check(lib().tba_debug_intr_cols(self._h, sizes.ctypes.data_as(C.POINTER(C.c_int64)), None))
+        n_slots, ni = (int(v) for v in sizes)
+        Ji = np.zeros((n_slots // 32, 2 * ni, 32))
+        self._check(lib().tba_debug_intr_cols(self._h, sizes.ctypes.data_as(C.POINTER(C.c_int64)), _dp(Ji)))
+        return Ji
 
     STREAM_KERNELS = ("linearize", "prepare", "matvec", "rhs_backsub")
 
